@@ -4,7 +4,7 @@ A "step" is ONE `model(batch)` call of the reference surface on synthetic pixels
 CLIP-ViT encoder -> visual projection -> image-row prefill of the 6 decoder layers -> KV-cached decode steps (max_len 40) ->
 search, i.e. the reference's `CaptioningModel.forward` in eval mode (reference layers/decoder.py:838-877, 977-1011).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--config 2|3|4|5] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--config 2|3|4|5] [--impl reference] [--dump-outputs DIR]
 
 --config names the BASELINE.json configuration (default 2 = the one the metric is quoted on):
   2  GIT_BASE,        64 images per call,            greedy   (BASELINE.json configs[1])
@@ -22,6 +22,8 @@ Numbers of a run (all with every call's full work inside the timed region):
             beside the per-call metric, never in place of it).
 Multi-GPU (torchrun, one rank per GPU): every rank captions its own batches (weak scaling, image-wise sharding, reference
 inference.py:165-169); the timed region ends with ONE fused NCCL all_gather of all finished token ids + logprobs.
+`--dump-outputs DIR` writes what the last timed `model(batch)` step returned (rank 0): DIR/predictions.npy (token ids as
+float64, exact) and DIR/logprobs.npy (float32).  Weights and pixels are seeded, so two builds can be compared output for output.
 `--impl reference` times the reference's own CPU algorithm (the as-shipped, no-KV-cache restatement in
 oracle/git_oracle.py -- the Python reference itself cannot travel to the GPU box) on the host cores.
 """
@@ -51,9 +53,8 @@ CONFIGS = {
             param=LARGE, batch=64, shard=1024, frames=0, search='greedy', cpu_sample=2,
             enc=dict(g=16, p=14, d=1024, layers=24, L=257)),
 }
-# threads of the CPU arm: measured on the pool's host (128 hardware threads, profiles/cpu_threads_probe_r02.txt): 8 threads
-# 0.79 s, 16 threads 0.53 s, 32 threads 1.11 s, 64 threads 2.41 s, 128 threads 112 s for the same B=2 / 9-step job --
-# intra-op parallelism of these small fp32 ops stops scaling at 16 threads and collapses beyond
+# threads of the CPU arm: intra-op parallelism of these small fp32 ops stops scaling at about 16 threads and collapses
+# beyond (more threads made the same job slower)
 CPU_THREADS_CAP = 16
 
 
@@ -71,16 +72,8 @@ def measured_peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d['hbm_gbs'], bf16_tflops=d['bf16_tflops'], bf16_sustained=d.get('bf16_tflops_sustained'),
                     source='measured (MEASURED_PEAKS.json)')
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_sustained=1400.0, source='fallback (B200_PROFILING.md)')
-
-
-def ncu_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel` from the committed `ncu --set full` captures
-    (profiles/roofline_traffic.json names the .ncu-rep extract each figure comes from)."""
-    p = os.path.join(ROOT, 'profiles', 'roofline_traffic.json')
-    if os.path.exists(p):
-        return json.load(open(p)).get(kernel, {}).get('dram_bytes_per_launch')
-    return None
+    # NVIDIA's H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 -- not reached figures
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_sustained=989.0, source='H100 SXM data sheet')
 
 
 def algorithmic_work(cfg):
@@ -103,8 +96,8 @@ def algorithmic_work(cfg):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md clocks line), streamed with
-    `-lms` so that even a sub-second region gets several samples."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries), streamed with `-lms` so that
+    even a sub-second region gets several samples."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -197,7 +190,7 @@ def run_reference_arm(args, cfg, rank):
                    'global_batch': sample, 'bench_config': args.config},
         'cpu_baseline': {'value': value, 'unit': UNIT, 'cores': threads, 'kind': 'port',
                          'host_cpus': os.cpu_count(),
-                         'threads_note': 'capped at %d: see profiles/cpu_threads_probe_r02.txt' % CPU_THREADS_CAP,
+                         'threads_note': 'capped at %d: intra-op parallelism of these small ops stops scaling there' % CPU_THREADS_CAP,
                          'sample': cpu_sample_text(cfg, sample, sec)},
         'e2e': {'value': value, 'unit': UNIT, 'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': 0},
     }
@@ -220,6 +213,8 @@ def main():
                     help='serving leg: engine launches in flight (the encoder of launch i+1 overlaps the decode loop of launch i)')
     ap.add_argument('--coalesce', type=int, default=4, choices=[1, 2, 3, 4],
                     help='serving leg: this many submitted batches share one engine launch (at most 256 decoder rows)')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='write the last timed step\'s predictions / logprobs as DIR/<name>.npy (float64 / float32)')
     ap.add_argument('--ncu-range', action='store_true',
                     help='bracket the timed region of `value` with cudaProfilerStart/Stop (use with ncu --profile-from-start off)')
     args = ap.parse_args()
@@ -323,14 +318,16 @@ def main():
         toks, lps = torch.cat(all_t, dim=0), torch.cat(all_l, dim=0)
         if world > 1:                        # ONE collective for everything this rank finished in the region
             toks, lps = gather_captions(toks.to(dev), lps.to(dev), toks.shape[0] * world)
-        return toks
+        return toks, lps
+
+    last = {}
 
     def timed(k, **kw):
         barrier()
         launches0 = model.launch_count()
         evs = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
         evs[0].record(stream)
-        toks = run(k, **kw)
+        toks, lps = run(k, **kw)
         torch.cuda.current_stream().wait_stream(stream)
         for sl in model._slots:          # the pipelined engines run on their own streams: join them before the end event
             if sl['stream'] is not None:
@@ -342,6 +339,9 @@ def main():
         if world > 1:
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
         assert toks.shape[0] == n_total * k and toks.shape[1] == MAX_STEPS, tuple(toks.shape)
+        # what the last step returned on every rank: the gathered rows are rank by rank, each rank's k steps in a row
+        last['predictions'] = toks.reshape(world, k, shard, -1)[:, -1].reshape(n_total, -1)
+        last['logprobs'] = lps.reshape(world, k, shard)[:, -1].reshape(n_total)
         return t.item(), model.launch_count() - launches0
 
     sampler = ClockSampler(local)
@@ -366,6 +366,11 @@ def main():
         if args.ncu_range:
             torch.cuda.profiler.stop()
         value = n_total * args.steps / (ms / 1e3)
+        if args.dump_outputs and rank == 0:
+            import numpy as np
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, 'predictions.npy'), last['predictions'].cpu().numpy().astype(np.float64))
+            np.save(os.path.join(args.dump_outputs, 'logprobs.npy'), last['logprobs'].float().cpu().numpy())
         # ---------------- `e2e`: the same calls with HOST pixels in, tokens + logprobs back ----------------
         run(2, to_host=True)
         ms_e2e, _ = timed(args.steps, to_host=True)
@@ -378,7 +383,7 @@ def main():
         if not args.no_serving and args.config != 5:
             co = max(1, min(args.coalesce, 256 // (B * beam)))
             depth = args.pipeline
-            k_serv = max(args.steps, 2 * depth * co)
+            k_serv = args.steps
             run(2 * depth * co, depth=depth, coalesce=co)
             ms_s, _ = timed(k_serv, depth=depth, coalesce=co)
             run(2 * depth * co, to_host=True, depth=depth, coalesce=co)
@@ -396,8 +401,7 @@ def main():
     roofline_gemm = None
     work = algorithmic_work(cfg)
     if rank == 0 and cfg['search'] == 'greedy':
-        # dominant kernel of a greedy call = decode_mega_kernel, one launch per decode step (profiles/launches_r02_*: ~2/3 of
-        # a config-2 call).  HBM bound: algorithmic bytes per launch = the bf16 decoder weights + LM head, the image K/V of
+        # dominant kernel of a greedy call = decode_mega_kernel, one launch per decode step.  HBM bound: algorithmic bytes per launch = the bf16 decoder weights + LM head, the image K/V of
         # every sequence and the text K/V so far (SURVEY.md 8d 'step bytes', averaged over the call's steps); duration =
         # CUDA events on the engine's stream around the call's decode loop / its step launches (gitb200_last_decode_ms).
         with torch.cuda.stream(stream):
@@ -407,16 +411,16 @@ def main():
             bytes_per_launch = work['decode_bytes'] / (MAX_STEPS - 1)
             avg_ms = ms_loop / n_launch
             achieved = bytes_per_launch / (avg_ms / 1e3) / 1e9
-            roofline = {'kernel': 'decode_mega_kernel (one persistent 148-CTA launch per decode step: 6 decoder layers + LM head + '
+            roofline = {'kernel': 'decode_mega_kernel (one persistent one-CTA-per-SM launch per decode step: 6 decoder layers + LM head + '
                                   'argmax / log-softmax + next embedding for %d sequences)' % B,
                         'bound': 'hbm', 'achieved': achieved, 'peak': peaks['hbm_gbs'], 'unit': 'GB/s',
-                        'frac': achieved / peaks['hbm_gbs'], 'traffic': ncu_traffic('decode_mega_kernel') if args.config == 2 else None,
+                        'frac': achieved / peaks['hbm_gbs'],
                         'avg_launch_ms': avg_ms, 'launches_timed': n_launch,
                         'algorithmic_bytes_per_launch': bytes_per_launch,
                         'peak_source': peaks['source'] + ', HBM copy bandwidth; the launches run back to back inside a call, '
                                        'so the figure includes the ~2 us between two graph launches'}
     if rank == 0 and not args.no_micro:
-        # dominant kernel = the tcgen05 GEMM family (profiles/: > 1/2 of a call); its largest instance is the ViT MLP c_fc
+        # dominant kernel of the encoder = the wgmma GEMM family; its largest instance is the ViT MLP c_fc
         # GEMM [images * L, d] x [d, 4d] (+bias +QuickGELU, bf16 out): algorithmic FLOPs = 2*M*N*K.
         e = cfg['enc']
         M, N, K = B * max(1, cfg['frames']) * e['L'], 4 * e['d'], e['d']
@@ -424,7 +428,7 @@ def main():
         w = (torch.randn(N, K, device=dev) * 0.03).to(torch.bfloat16)
         bias = torch.randn(N, device=dev)
         out = torch.empty(M, N, dtype=torch.bfloat16, device=dev)
-        flush = torch.empty(160 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 126 MB L2
+        flush = torch.empty(160 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 50 MB L2
         with torch.cuda.stream(stream):
             def gemm():
                 rc = lib.gitb200_op_gemm(a.data_ptr(), w.data_ptr(), bias.data_ptr(), None, out.data_ptr(), M, N, K, 1, 1, 0, 1,
@@ -444,9 +448,9 @@ def main():
         avg_ms = sum(durs) / len(durs)
         flops = 2.0 * M * N * K
         achieved = flops / (avg_ms / 1e3) / 1e12
-        roofline_gemm = {'kernel': 'gemm2_bf16_tcgen05<256> (ViT mlp.c_fc shape %dx%dx%d, bias+QuickGELU epilogue)' % (M, N, K),
+        roofline_gemm = {'kernel': 'gemm_bf16_wgmma<256> (ViT mlp.c_fc shape %dx%dx%d, bias+QuickGELU epilogue)' % (M, N, K),
                     'bound': 'tensor', 'achieved': achieved, 'peak': peaks['bf16_tflops'], 'unit': 'TFLOP/s',
-                    'frac': achieved / peaks['bf16_tflops'], 'traffic': ncu_traffic('gemm2_bf16_tcgen05') if args.config == 2 else None,
+                    'frac': achieved / peaks['bf16_tflops'],
                     'avg_launch_ms': avg_ms,
                     'peak_source': peaks['source'] + ', burst bf16 figure (kernel timed alone, L2 flushed between launches)'}
     # whole-call roofline (SURVEY.md section 8d): tensor part at the sustained GEMM peak + decode bytes at the HBM peak
@@ -477,7 +481,7 @@ def main():
                        'bench_config': args.config, 'global_batch': n_total, 'per_gpu_batch': shard,
                        'parallelism': 'image-parallel x%d, ONE fused all_gather of the finished captions per timed region' % world,
                        'l2': 'inputs larger than L2: every call streams the bf16 weights (%.2f GB) + the image K/V cache per step '
-                             '(>> 126 MB); no flush needed between steps' % (0.31 if cfg['model'] != 'GIT_LARGE' else 0.74),
+                             '(>> 50 MB); no flush needed between steps' % (0.31 if cfg['model'] != 'GIT_LARGE' else 0.74),
                        'compute': 'bf16 operands, fp32 accumulate, fp32 residual stream',
                        'calls': 'one model(batch) at a time (SURVEY.md 8d); the dynamic-batching form is under "serving"'},
             'e2e': {'value': e2e_value, 'unit': UNIT, 'ms_per_step': ms_e2e / args.steps, 'h2d_bytes_per_step': h2d_bytes,

@@ -5,7 +5,7 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, 'libgitb200.so')
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 c_void_p, c_int, c_int64, c_float, c_char_p = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_char_p
 c_ll = ctypes.c_longlong

@@ -3,32 +3,33 @@
 // (reference layers/decoder.py:313-417, 65-78; layers/bert/modeling_bert.py:92-334) -- replacing the 45-launch chain of
 // gitb200.cu::step_layers for that case.
 //
-// Why: at <= 64 rows every kernel of the chain is latency bound (TMA -> tcgen05 -> TMEM -> epilogue -> flag, ~7 us per
-// hop, ~400 us per step against an HBM floor of ~50 us).  Here the HBM stream is decoupled from the dependency chain:
-//   * 148 CTAs (one per SM, cooperative launch), 8 compute warps + 1 producer warp each;
+// Why: at <= 64 rows every kernel of the chain is latency bound (TMA -> tensor core -> epilogue -> flag per hop, far above
+// the HBM floor of the step's weight bytes).  Here the HBM stream is decoupled from the dependency chain:
+//   * one CTA per SM (132 on an H100; cooperative launch), 8 compute warps + 1 producer warp each;
 //   * every byte the step reads from HBM -- the weight tiles a CTA owns in each GEMM phase, the image K/V of its attention
 //     items and the text K/V so far -- flows through a 12 x 16 KB shared-memory ring that the producer warp fills in
 //     program order with TMA (bulk copies of pre-packed weight tiles, 64-key swizzled K | V box pairs), running as far
 //     ahead of the compute warps as the ring allows, across phase boundaries (only the text K/V of the CURRENT layer waits
 //     for that layer's QKV phase);
 //   * phases (QKV | attention | out-proj | LN | fc1 | fc2 | LN per layer, then LM head | selection + embedding) are
-//     separated by a grid barrier (one release-add + acquire-spin on a global counter, 1.7 us on B200 -- the cheapest of
+//     separated by a grid barrier (one release-add + acquire-spin on a global counter -- the cheapest of
 //     the variants tools/barrier_bench.cu times); what crosses a barrier is only the <= 64-row activations, read straight
 //     from L2 into mma.sync fragments;
 //   * weights are stationary per CTA: a GEMM phase gives CTA c a few 8-feature tiles over a 768-long reduction; the 8 warps
-//     split a tile 4 row tiles x 2 K halves.  fc2 (K = 3072) is dealt as 4 k slices x 96 feature tiles over 128 CTAs, its
+//     split a tile 4 row tiles x 2 K halves.  The 288 q | k | v tiles go out two per CTA, three for the first 288 - 2G.  fc2 (K = 3072) is dealt as 4 k slices x 96 feature tiles over 128 CTAs, its
 //     four partial sums meet in slice order in the LayerNorm phase: no atomics anywhere, the step is bit-reproducible;
 //   * attention: the 64-key chunks of a CTA's (sequence, head) items are dealt round-robin to its 8 warps, online-softmax
 //     states in shared memory, fixed-order merge.
 // The skinny GEMMs and the 1-row attention are HBM-bound byte work (arithmetic intensity ~rows FLOP/B): they use the
-// warp-level mma.sync path fed from shared memory (measured limit here: ~0.77 us per 64 x 8 x 768 tile per SM, which is
-// what the 26-tile LM-head slice of a CTA costs); tcgen05 / TMEM stay with the compute-bound encoder and prefill GEMMs:
-// with the weights as the M operand a tcgen05 tile needs >= 64 weight rows per CTA (3/4 of the SMs, and of the HBM stream,
+// warp-level mma.sync path fed from shared memory; wgmma stays with the compute-bound encoder and prefill GEMMs:
+// with the weights as the M operand a wgmma tile needs >= 64 weight rows per CTA (3/4 of the SMs, and of the HBM stream,
 // would idle in the layer GEMMs); with the activations as the M operand every CTA would have to stage the 64 x 768
 // activations (96 KB) in shared memory in every phase, which the 192 KB ring leaves no room for.
 #pragma once
 #include "ptx.cuh"
 #include "rowops.cuh"
+
+#include <type_traits>
 
 namespace gitb200 {
 
@@ -40,7 +41,9 @@ constexpr int kMegaTileBytes = 12288;      // 8 output features x 768 k x bf16, 
 constexpr int kMegaKvRows = 64;            // keys per attention chunk: one ring slot = K box (8 KB) | V box (8 KB)
 constexpr int kMegaMaxRows = 64;
 constexpr int kMegaD = 768, kMegaF = 3072, kMegaH = 12;
-constexpr int kMegaAttItems = 6;           // (sequence, head) attention items of the busiest CTA: ceil(64 * 12 / 148)
+constexpr int kMegaAttItems = 6;           // (sequence, head) attention items of the busiest CTA: ceil(64 * 12 / 132)
+constexpr int kMegaMinCtas = 128;          // fc1 / fc2 deal their tiles over 128 CTAs; attention needs ceil(64 * 12 / G) <= 6
+constexpr int kMegaQkvTiles = 288;         // q | k | v: 2304 features in 8-feature tiles, 2-3 per CTA (needs G >= 96)
 constexpr int kMegaAttState = 72;          // floats per (item, warp) softmax state: 64 output dims, running max, 4 lane sums
 constexpr unsigned int kMegaSpinLimit = 1u << 18;   // bounded waits: a protocol bug must end in an error code, not a hung device
 
@@ -85,9 +88,8 @@ struct MegaParams {
 // Tile layout: 48 k-steps x 32 lanes x 8 bytes.  Lane (g = lane / 4, t = lane % 4) of k-step s holds the four k values
 // k0 + 64 * (s / 4) + 16 t + 4 (s % 4) + {0, 1, 2, 3} of feature 8 tile + g: the B fragment (b0 = first pair, b1 = second
 // pair) of an m16n8k16 MMA whose k index has been permuted so that the matching A fragment is 16 CONTIGUOUS bf16 per
-// thread and group of four k-steps -- one 256-bit load from the row-major activation matrix, and the four lanes of a row
-// together fetch one whole 128-byte line (with 128-bit loads every line was touched by two instructions, and the L1
-// wavefronts of the A loads, not L2 bandwidth, set the pace of the GEMM phases: profiles/decode_mega_timeline_r02_call18.txt).
+// thread and group of four k-steps -- 32 contiguous bytes of the row-major activation matrix, and the four lanes of a row
+// together fetch one whole 128-byte line.
 __global__ void __launch_bounds__(256) pack_tiles_kernel(const __nv_bfloat16* __restrict__ W, long long ldw, int n_feat, int k0,
                                                          uint8_t* __restrict__ dst, long long n_tiles, int tile_stride_tiles,
                                                          int tile_offset) {
@@ -148,9 +150,6 @@ struct MegaTl {
 __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 // false: gave up (or another wait already had: once the error word is set every further wait returns at once, so a broken
 // launch drains in microseconds instead of timing out chunk by chunk)
@@ -215,8 +214,8 @@ __device__ __forceinline__ void mega_grid_sync(unsigned int* counter, unsigned i
     if (tl_id) tlf.mark(tl_id + 6);                                 // all compute warps of the CTA are here
     else tl_mark_one(500000 + static_cast<int>(epoch / gridDim.x)); // this CTA arrived at barrier #n
     // release-RMW at gpu scope: cumulative over the CTA's writes that the bar.sync above ordered before this thread, so
-    // no separate fence -- __threadfence() is a sequentially-consistent fence (MEMBAR.SC.GPU + L1 invalidate) that cost
-    // 0.5-2.5 us per barrier here on top of the release's own MEMBAR.ALL.GPU
+    // no separate fence -- __threadfence() is a sequentially-consistent fence (MEMBAR.SC.GPU + L1 invalidate) that would
+    // come on top of the release's own MEMBAR.ALL.GPU
     if (tl_id) tlf.mark(tl_id + 7);
     asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(counter), "r"(1u) : "memory");
     if (tl_id) tlf.mark(tl_id + 8);
@@ -239,10 +238,12 @@ struct MegaAFrag {
   uint32_t lo[6][8];   // row g     : 16 contiguous k per entry (four k-steps)
   uint32_t hi[6][8];   // row g + 8
 };
+// 32 contiguous bytes, L1-bypassing (sm_90 has no 256-bit loads: two 128-bit ones)
 __device__ __forceinline__ void ldcg_256(uint32_t (&r)[8], const void* p) {
-  asm volatile("ld.global.cg.v8.u32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "l"(p));
+  asm volatile("ld.global.cg.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "l"(p));
+  asm volatile("ld.global.cg.v4.u32 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
+               : "l"(static_cast<const uint8_t*>(p) + 16));
 }
 __device__ __forceinline__ void mega_load_a(MegaAFrag& a, const __nv_bfloat16* A, long long lda, int rows, int mt, int kh, int lane) {
   const int g = lane >> 2, t = lane & 3;
@@ -367,6 +368,10 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
   const int lm_per = (lm_tiles_total + G - 1) / G;
   const int lm_t0 = cta * lm_per;
   const int lm_n = max(0, min(lm_per, lm_tiles_total - lm_t0));
+  // q | k | v tiles of this CTA, one pass: two each, three for the first 288 - 2G CTAs when G < 144 (contiguous ranges)
+  const int qkv_extra = max(0, kMegaQkvTiles - 2 * G);
+  const int qkv_t0 = (cta < qkv_extra) ? 3 * cta : 2 * cta + qkv_extra;
+  const int qkv_n = (cta < qkv_extra) ? 3 : max(0, min(2, kMegaQkvTiles - qkv_t0));
 
   if (tid == 0) {
     tma_prefetch_desc(&tmKV);
@@ -411,7 +416,7 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
       };
       for (int l = 0; l < p.n_layers; ++l) {
         const MegaLayer& L = p.layer[l];
-        if (cta < 144) for (int j = 0; j < 2; ++j) tile(L.wqkv + static_cast<size_t>(cta * 2 + j) * kMegaTileBytes);
+        for (int j = 0; j < qkv_n; ++j) tile(L.wqkv + static_cast<size_t>(qkv_t0 + j) * kMegaTileBytes);
         // attention chunks ("units") of this CTA's items, round-major: unit u = r * n_my_items + k is keys 64r .. 64r + 63 of
         // item k (image keys first, then the text rounds); the consumer deals the units to its 8 warps round-robin
         for (int r = 0; r < n_kv + n_txt; ++r) {
@@ -466,26 +471,32 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
   for (int l = 0; l < p.n_layers; ++l) {
     const MegaLayer& L = p.layer[l];
     // ------------------------------------------------ P1: q | k | v ------------------------------------------------
-    if (cta < 144) {
+    auto qkv_tiles = [&](auto nt) {
+      constexpr int NT = decltype(nt)::value;
       MegaAFrag a;
       if (MEGA_TL_ID(1)) tlf.mark(MEGA_TL_ID(1) + 0);
       mega_load_a(a, p.hb, kMegaD, R, mt, kh, lane);
       if (MEGA_TL_ID(1)) { tlf.mark(MEGA_TL_ID(1) + 1); MEGA_TL_DEP(a) tlf.mark(MEGA_TL_ID(1) + 2); }
-      float2 bias_j[2];
+      float2 bias_j[NT];
 #pragma unroll
-      for (int j = 0; j < 2; ++j) bias_j[j] = __ldg(reinterpret_cast<const float2*>(L.bqkv + (cta * 2 + j) * 8 + 2 * t));
-      float c[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-      const uint8_t* tb[2] = {rg.acquire_ahead(0), rg.acquire_ahead(1)};
+      for (int j = 0; j < NT; ++j) bias_j[j] = __ldg(reinterpret_cast<const float2*>(L.bqkv + (qkv_t0 + j) * 8 + 2 * t));
+      float c[NT][4];
+      const uint8_t* tb[NT];
+#pragma unroll
+      for (int j = 0; j < NT; ++j) {
+        c[j][0] = c[j][1] = c[j][2] = c[j][3] = 0.f;
+        tb[j] = rg.acquire_ahead(j);
+      }
       if (MEGA_TL_ID(1)) tlf.mark(MEGA_TL_ID(1) + 3);
-      mega_mma_tiles<2>(c, a, tb, kh, lane);
-      rg.release();
-      rg.release();
-      const bool own1 = mega_combine_n<2>(c, redv, red_buf, mt, kh, lane);
+      mega_mma_tiles<NT>(c, a, tb, kh, lane);
+#pragma unroll
+      for (int j = 0; j < NT; ++j) rg.release();
+      const bool own1 = mega_combine_n<NT>(c, redv, red_buf, mt, kh, lane);
       if (MEGA_TL_ID(1)) tlf.mark(MEGA_TL_ID(1) + 4);
       if (own1) {
 #pragma unroll
-        for (int j = 0; j < 2; ++j) {
-          const int f = (cta * 2 + j) * 8 + 2 * t;
+        for (int j = 0; j < NT; ++j) {
+          const int f = (qkv_t0 + j) * 8 + 2 * t;
           const float2 bias = bias_j[j];
           const int seg = f / kMegaD, fo = f - seg * kMegaD;
 #pragma unroll
@@ -503,7 +514,9 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
         }
       }
       red_buf ^= 1;
-    }
+    };
+    if (qkv_n == 3) qkv_tiles(std::integral_constant<int, 3>());
+    else if (qkv_n == 2) qkv_tiles(std::integral_constant<int, 2>());
     mega_grid_sync(bar, epoch, p.error, tlf, MEGA_TL_ID(1));
     // ------------------------------------------------ P2: attention ------------------------------------------------
     // The CTA's 5-6 (sequence, head) items x (image + text) 64-key chunks form U units; warp w takes units w, w + 8, ...

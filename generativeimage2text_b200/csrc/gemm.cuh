@@ -1,12 +1,11 @@
 // C[M,N] = A[M,K] * B[N,K]^T with bf16 operands (both K-major: exactly the layout of an activation
-// matrix and of an nn.Linear weight), fp32 accumulation in TMEM, fused epilogues.
+// matrix and of an nn.Linear weight), fp32 accumulation in registers (wgmma), fused epilogues.
 //
-// One persistent, warp-specialised sm_100a kernel:
-//   warp 0   : TMA producer  (cp.async.bulk.tensor, 128B-swizzled [rows x 64] bf16 tiles, STAGES-deep ring)
-//   warp 1   : UMMA issuer   (one lane issues tcgen05.mma 128 x BN x 16, accumulators double-buffered in TMEM)
-//   warp 2   : TMEM allocator
-//   warps 4-7: epilogue      (tcgen05.ld -> bias / activation / residual -> global stores)
-// so the epilogue of tile i overlaps the main loop of tile i+1.
+// One persistent, warp-specialised sm_90a kernel per tile width BN, 128 x BN output tiles:
+//   warpgroup 0    : TMA producer (one thread: cp.async.bulk.tensor, 128B-swizzled [rows x 64] bf16 tiles, STAGES-deep ring)
+//   warpgroups 1-2 : MMA + epilogue, 64 tile rows each (wgmma m64nBNk16 from shared memory, one wgmma group in flight
+//                    while the next k-block is issued); the epilogue stages 64 x 64 fp32 chunks in shared memory
+// so the producer streams the next tile's operands while the MMA warpgroups run the epilogue of this one.
 //
 // Two epilogue shapes:
 //   normal     : out[row_map(m)][n] (+bias[n]) (+act) (+resid[m][n]); N may be split into up to three equal
@@ -65,22 +64,23 @@ struct GemmCfg {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int EPI_WARPS = 8;                       // two per TMEM lane quadrant
-  static constexpr int THREADS = 128 + EPI_WARPS * 32;      // warps 0-3: TMA / MMA / TMEM alloc / spare
-  static constexpr int STAGING_BYTES = EPI_WARPS * 32 * 128;  // per warp: 32 rows x 32 fp32, 16B-chunk XOR swizzle
+  static constexpr int MMA_WGS = 2;                          // 64 tile rows each
+  static constexpr int THREADS = 128 * (1 + MMA_WGS);        // warpgroup 0: TMA producer
+  static constexpr int WG_STAGING_BYTES = 4 * 32 * 128;     // per MMA warpgroup: 64 rows x 64 fp32 as four 32 x 32 blocks
+  static constexpr int STAGING_BYTES = MMA_WGS * WG_STAGING_BYTES;
   static constexpr int BAR_BYTES = 256;
   static constexpr int SMEM_LIMIT = 227 * 1024;
   static constexpr int STAGES_RAW = (SMEM_LIMIT - 1024 - BAR_BYTES - STAGING_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-  static constexpr int TMEM_COLS = (2 * BN <= 128) ? 128 : ((2 * BN <= 256) ? 256 : 512);
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + 1024 + BAR_BYTES;
-  static_assert(BN % 32 == 0 && BN >= 32 && BN <= 256, "BN");
+  static constexpr int PRODUCER_REGS = 40, MMA_REGS = 232;  // 128 x 40 + 256 x 232 <= 64 K registers
+  static_assert(BN % 64 == 0 && BN >= 64 && BN <= 256, "BN");
   static_assert(B_BYTES % 1024 == 0, "B tile must keep 1024B alignment for SWIZZLE_128B");
-  static_assert((2 * STAGES + 4) * 8 + 8 <= BAR_BYTES, "barrier area");
+  static_assert(2 * STAGES * 8 <= BAR_BYTES, "barrier area");
   static_assert(STAGES >= 3, "pipeline depth");
 };
 
-// ---- epilogue building blocks shared by the 1-CTA kernel below and the CTA-pair kernel of gemm2.cuh --------------------
+// ---- epilogue building blocks ---------------------------------------------------------------------------------------------
 // Output row offsets (elements) of the 8 rows a lane stores in the normal epilogue: rows row0 + it * 4 + (lane >> 3).
 __device__ __forceinline__ uint32_t epi_row_offsets(const GemmParams& p, int row0, int rsub, bool store_ok, long long (&ooff)[8]) {
   uint32_t okmask = 0;
@@ -96,11 +96,11 @@ __device__ __forceinline__ uint32_t epi_row_offsets(const GemmParams& p, int row
   return okmask;
 }
 
-// Normal epilogue of one 32x32 fp32 accumulator chunk (thread = row after tcgen05.ld): transpose through the warp's
-// swizzled staging buffer so that each lane ends up with 4 consecutive output elements of one row (coalesced 128-bit
-// accesses), then (+bias) (+act) (+residual) -> bf16 / fp32 stores into the chunk's column segment.
+// Normal epilogue of one 32x32 fp32 accumulator chunk staged in the warp's swizzled buffer as [row][column] (16-byte
+// chunk j of row r at r * 128 + ((j ^ (r & 7)) << 4)): each lane takes 4 consecutive output elements of one row
+// (coalesced 128-bit accesses), then (+bias) (+act) (+residual) -> bf16 / fp32 stores into the chunk's column segment.
 template <int EPI>
-__device__ __forceinline__ void epi_store_normal(const GemmParams& p, const uint32_t (&r)[32], uint8_t* stg, int lane, int n0,
+__device__ __forceinline__ void epi_store_normal(const GemmParams& p, const uint8_t* stg, int lane, int n0,
                                                  int row0, const long long (&ooff)[8], uint32_t okmask) {
   constexpr bool kBf16 = (EPI & EPI_BF16) != 0;
   constexpr bool kResid = (EPI & EPI_RESID) != 0;
@@ -109,12 +109,7 @@ __device__ __forceinline__ void epi_store_normal(const GemmParams& p, const uint
   static_assert(!kSplit3 || kBf16, "split3 is a bf16 output format");
   const int c4 = lane & 7;
   const int rsub = lane >> 3;
-  // phase 1: thread = row; 8 x STS.128, chunk position XOR-swizzled by the row
-#pragma unroll
-  for (int j = 0; j < 8; ++j)
-    *reinterpret_cast<uint4*>(stg + lane * 128 + ((j ^ (lane & 7)) << 4)) = make_uint4(r[4 * j], r[4 * j + 1], r[4 * j + 2], r[4 * j + 3]);
-  __syncwarp();
-  // phase 2: 8 lanes per row (4 columns each), 4 rows per instruction
+  // 8 lanes per row (4 columns each), 4 rows per instruction
   float4 b4 = make_float4(0.f, 0.f, 0.f, 0.f);
   if (p.bias != nullptr) b4 = __ldg(reinterpret_cast<const float4*>(p.bias + n0) + c4);
   int seg = 0;
@@ -165,19 +160,90 @@ __device__ __forceinline__ void epi_store_normal(const GemmParams& p, const uint
       }
     }
   }
-  __syncwarp();
 }
 
-template <int BN, int EPI>
-__global__ void __launch_bounds__(GemmCfg<BN>::THREADS, 1)
-gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const GemmParams p) {
-  using C = GemmCfg<BN>;
-  constexpr bool kTransposed = (EPI & EPI_TRANSPOSED) != 0;
+// Transposed ("swap-AB") epilogue of one 32x32 chunk staged as [activation row][feature] (16-byte chunk j of row r at
+// r * 128 + ((j ^ (r & 7)) << 4)): each lane owns 4 consecutive features of one activation row -- 128-bit stores.
+// row0 = first feature (A row) of the chunk, n0 = first activation row (B row).
+template <int EPI>
+__device__ __forceinline__ void epi_store_transposed(const GemmParams& p, const uint8_t* stg, int lane, int n0, int row0,
+                                                     int split, bool store_ok) {
   constexpr bool kBf16 = (EPI & EPI_BF16) != 0;
   constexpr bool kPartial = (EPI & EPI_PARTIAL) != 0;
   constexpr int kAct = (EPI >> EPI_ACT_SHIFT) & 3;
   constexpr bool kSplit3 = (EPI & EPI_SPLIT3) != 0;
+  const int c4 = lane & 7;
+  const int rsub = lane >> 3;
+  const int f0 = row0 + c4 * 4;  // first of this lane's 4 features
+  const bool full4 = (f0 + 3) < p.M;
+  float bv[4] = {0.f, 0.f, 0.f, 0.f};
+  if (p.bias != nullptr && split == 0) {
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+      if (f0 + e < p.M) bv[e] = __ldg(p.bias + f0 + e);
+  }
+#pragma unroll
+  for (int it = 0; it < 8; ++it) {
+    const int rr = it * 4 + rsub;
+    const int arow = n0 + rr;
+    const float4 t4 = *reinterpret_cast<const float4*>(stg + rr * 128 + ((c4 ^ (rr & 7)) << 4));
+    float v[4] = {t4.x + bv[0], t4.y + bv[1], t4.z + bv[2], t4.w + bv[3]};
+    if (kAct != ACT_NONE) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) v[e] = act_ct<kAct>(v[e]);
+    }
+    if (arow < p.N && store_ok && f0 < p.M) {
+      const long long off = static_cast<long long>(arow) * p.ldo + f0;
+      if (kPartial) {   // this split's own partial-sum buffer (plain stores; summed in split order by the consumer)
+        float* dst = reinterpret_cast<float*>(p.out[0]) + static_cast<long long>(split) * p.split_stride + off;
+        if (full4 && (p.ldo & 3) == 0) {
+          *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
+        } else {
+          for (int e = 0; e < 4; ++e)
+            if (f0 + e < p.M) dst[e] = v[e];
+        }
+      } else if (kSplit3) {
+        __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.out[0]) + off;
+        for (int e = 0; e < 4; ++e) {
+          if (f0 + e < p.M) {
+            __nv_bfloat16 hi, lo;
+            split_bf16(v[e], hi, lo);
+            dst[e] = hi; dst[p.M + e] = lo; dst[2 * p.M + e] = hi;
+          }
+        }
+      } else if (kBf16) {
+        __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.out[0]) + off;
+        if (full4 && (p.ldo & 3) == 0) {
+          uint2 pk;
+          pk.x = pack_bf16(v[0], v[1]);
+          pk.y = pack_bf16(v[2], v[3]);
+          *reinterpret_cast<uint2*>(dst) = pk;
+        } else {
+          for (int e = 0; e < 4; ++e)
+            if (f0 + e < p.M) dst[e] = __float2bfloat16_rn(v[e]);
+        }
+      } else {
+        float* dst = reinterpret_cast<float*>(p.out[0]) + off;
+        if (full4 && (p.ldo & 3) == 0) {
+          *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
+        } else if (full4 && (p.ldo & 1) == 0) {
+          *reinterpret_cast<float2*>(dst) = make_float2(v[0], v[1]);
+          *reinterpret_cast<float2*>(dst + 2) = make_float2(v[2], v[3]);
+        } else {
+          for (int e = 0; e < 4; ++e)
+            if (f0 + e < p.M) dst[e] = v[e];
+        }
+      }
+    }
+  }
+}
+
+template <int BN, int EPI>
+__global__ void __launch_bounds__(GemmCfg<BN>::THREADS, 1)
+gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                const GemmParams p) {
+  using C = GemmCfg<BN>;
+  constexpr bool kTransposed = (EPI & EPI_TRANSPOSED) != 0;
   if (p.pdl) griddep_launch_early();
   if (p.pdl) tl_mark(100000 + 1000 + static_cast<int>(gridDim.x));
   // `skip` (decode finished) only changes between steps, which are separated by full dependencies
@@ -190,36 +256,21 @@ gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   uint8_t* sStage = smem + C::STAGES * C::STAGE_BYTES;
   uint64_t* full = reinterpret_cast<uint64_t*>(sStage + C::STAGING_BYTES);
   uint64_t* empty = full + C::STAGES;
-  uint64_t* tfull = empty + C::STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
 
-  const int warp = threadIdx.x >> 5;
+  const int wg = threadIdx.x >> 7;
+  const int warp = (threadIdx.x >> 5) & 3;   // warp within its warpgroup
   const int lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < C::STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull[a], 1);
-      mbar_init(&tempty[a], C::EPI_WARPS);
+      mbar_init(&empty[s], C::MMA_WGS);   // one arrive per MMA warpgroup once its wgmmas have read the slot
     }
     mbar_fence_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, C::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int m_tiles = (p.M + C::BM - 1) / C::BM;
   const int n_tiles = (p.N + BN - 1) / BN;
@@ -236,7 +287,7 @@ gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int split = static_cast<int>(blockIdx.x) / mn_tiles;
     const int kb0 = split * kb_per;
     npre = min(C::STAGES, min(kb_total, kb0 + kb_per) - kb0);
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
       const int m_blk = (static_cast<int>(blockIdx.x) - split * mn_tiles) / n_tiles;
       for (int i = 0; i < npre; ++i) {
         mbar_arrive_expect_tx(&full[i], C::STAGE_BYTES);
@@ -248,9 +299,10 @@ gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   else if (p.pdl) griddep_wait();
   if (p.pdl) tl_mark(1000 + static_cast<int>(gridDim.x));
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ------------------------------ TMA producer ------------------------------
-    if (lane == 0) {
+    setmaxnreg_dec<C::PRODUCER_REGS>();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -277,167 +329,90 @@ gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------ UMMA issuer -------------------------------
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(C::BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int accum = 0;
-      uint32_t accum_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int split = tile / mn_tiles;
-        const int kb0 = split * kb_per;
-        const int kb1 = min(kb_total, kb0 + kb_per);
-        mbar_wait(&tempty[accum], accum_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + accum * BN;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          if (p.pdl && tile == static_cast<int>(blockIdx.x) && kb == kb0) tl_mark_one(300000 + 1000 + static_cast<int>(gridDim.x));
-          const uint32_t a_base = smem_u32(sA + stage * C::A_BYTES);
-          const uint32_t b_base = smem_u32(sB + stage * C::B_BYTES);
-#pragma unroll
-          for (int k = 0; k < C::BK / 16; ++k) {
-            umma_bf16(d_tmem, umma_desc_sw128(a_base + k * 32), umma_desc_sw128(b_base + k * 32), idesc,
-                      (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty[stage]);  // frees the smem slot once these MMAs have read it
-          if (++stage == C::STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tfull[accum]);  // accumulator complete -> epilogue
-        accum ^= 1;
-        if (accum == 0) accum_phase ^= 1;
-      }
-    }
-  } else if (warp >= 4) {
-    // ------------------------------ epilogue ----------------------------------
-    // 8 warps: warp w reads TMEM lanes 32*(w%4).. (hardware restriction) and the 32-column chunks
-    // c == (w-4)/4 (mod 2).  Every 32x32 fp32 chunk is transposed through a per-warp swizzled staging buffer so
-    // that each lane ends up with 4 consecutive output elements of one row: coalesced 128-bit accesses.
-    const int q = warp & 3;
-    const int half = (warp - 4) >> 2;
+  } else {
+    // ------------------------------ MMA + epilogue ----------------------------
+    setmaxnreg_inc<C::MMA_REGS>();
+    const int mw = wg - 1;                                   // rows 64 mw .. 64 mw + 63 of the tile
     const bool store_ok = !(p.pdl && !chained && p.skip != nullptr && *p.skip != 0);  // finished decode: no stores
-    uint8_t* stg = sStage + (warp - 4) * (32 * 128);
-    const int c4 = lane & 7;
+    uint8_t* stg_wg = sStage + mw * C::WG_STAGING_BYTES;
+    uint8_t* stg = stg_wg + warp * (32 * 128);              // the 32 x 32 block this warp stores
     const int rsub = lane >> 3;
-    int accum = 0;
-    uint32_t accum_phase = 0;
+    float acc[BN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int split = tile / mn_tiles;
       const int rem = tile - split * mn_tiles;
       const int m_blk = rem / n_tiles;
       const int n_blk = rem - m_blk * n_tiles;
-      const int row0 = m_blk * C::BM + q * 32;  // first tile row of this warp
-      // ---- per-tile row bookkeeping (normal mode): output row offsets of this lane's 8 rows ----
+      const int kb0 = split * kb_per;
+      const int kb1 = min(kb_total, kb0 + kb_per);
+      int prev = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full[stage], phase);
+        if (p.pdl && tile == static_cast<int>(blockIdx.x) && kb == kb0 && threadIdx.x == 128) tl_mark_one(300000 + 1000 + static_cast<int>(gridDim.x));
+        const uint32_t a_base = smem_u32(sA + stage * C::A_BYTES + mw * (64 * 128));
+        const uint32_t b_base = smem_u32(sB + stage * C::B_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < C::BK / 16; ++k)
+          Wgmma<BN>::mma(acc, wgmma_desc_sw128(a_base + k * 32), wgmma_desc_sw128(b_base + k * 32), (kb > kb0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        if (prev >= 0) {   // the previous k-block's wgmmas have read their slot: free it
+          wgmma_wait<1>();
+          if ((threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+        }
+        prev = stage;
+        if (++stage == C::STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      wgmma_wait<0>();
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+      if (p.pdl && tile == static_cast<int>(blockIdx.x) && threadIdx.x == 128) tl_mark_one(400000 + 1000 + static_cast<int>(gridDim.x));
+
+      // ---- epilogue: 64-column chunks through the warpgroup's staging buffer (block b = 2 * column half + row half,
+      //      [row][column] in the normal shape, [column][row] in the transposed one); warp w then stores block w ----
+      const int row0 = m_blk * C::BM + mw * 64 + (warp & 1) * 32;   // first tile row of this warp's block
       long long ooff[8];
       uint32_t okmask = 0;
       if (!kTransposed) okmask = epi_row_offsets(p, row0, rsub, store_ok, ooff);
-      mbar_wait(&tfull[accum], accum_phase);
-      tc_fence_after();
-      if (p.pdl && tile == static_cast<int>(blockIdx.x) && warp == 4 && lane == 0) tl_mark_one(400000 + 1000 + static_cast<int>(gridDim.x));
-#pragma unroll 1
-      for (int c = half; c < BN / 32; c += 2) {
-        const int n0 = n_blk * BN + c * 32;
-        if (n0 >= p.N) break;  // warp-uniform
-        uint32_t r[32];
-        tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + accum * BN + c * 32, r);
-        tmem_ld_wait();
-        if (!kTransposed) {
-          epi_store_normal<EPI>(p, r, stg, lane, n0, row0, ooff, okmask);
-        } else {
-          // transposed ("swap-AB"): lane = output feature, register j = activation row n0 + j.  Stage the 32x32
-          // chunk as [activation row][feature] so that each lane then owns 4 consecutive features of one row:
-          // 128-bit stores / vector reductions (a warp-wide scalar RED costs ~1.3 cycles per lane on the LSU).
 #pragma unroll
-          for (int j = 0; j < 32; ++j)
-            *reinterpret_cast<uint32_t*>(stg + j * 128 + (((lane >> 2) ^ (j & 7)) << 4) + ((lane & 3) << 2)) = r[j];
-          __syncwarp();
-          const int f0 = row0 + c4 * 4;  // first of this lane's 4 features
-          const bool full4 = (f0 + 3) < p.M;
-          float bv[4] = {0.f, 0.f, 0.f, 0.f};
-          if (p.bias != nullptr && split == 0) {
+      for (int cc = 0; cc < BN / 64; ++cc) {
+        if (n_blk * BN + cc * 64 >= p.N) break;   // uniform over the warpgroup
 #pragma unroll
-            for (int e = 0; e < 4; ++e)
-              if (f0 + e < p.M) bv[e] = __ldg(p.bias + f0 + e);
-          }
+        for (int j8 = 0; j8 < 8; ++j8) {
 #pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int rr = it * 4 + rsub;
-            const int arow = n0 + rr;
-            const float4 t4 = *reinterpret_cast<const float4*>(stg + rr * 128 + ((c4 ^ (rr & 7)) << 4));
-            float v[4] = {t4.x + bv[0], t4.y + bv[1], t4.z + bv[2], t4.w + bv[3]};
-            if (kAct != ACT_NONE) {
-#pragma unroll
-              for (int e = 0; e < 4; ++e) v[e] = act_ct<kAct>(v[e]);
-            }
-            if (arow < p.N && store_ok && f0 < p.M) {
-              const long long off = static_cast<long long>(arow) * p.ldo + f0;
-              if (kPartial) {   // this split's own partial-sum buffer (plain stores; summed in split order by the consumer)
-                float* dst = reinterpret_cast<float*>(p.out[0]) + static_cast<long long>(split) * p.split_stride + off;
-                if (full4 && (p.ldo & 3) == 0) {
-                  *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
-                } else {
-                  for (int e = 0; e < 4; ++e)
-                    if (f0 + e < p.M) dst[e] = v[e];
-                }
-              } else if (kSplit3) {
-                __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.out[0]) + off;
-                for (int e = 0; e < 4; ++e) {
-                  if (f0 + e < p.M) {
-                    __nv_bfloat16 hi, lo;
-                    split_bf16(v[e], hi, lo);
-                    dst[e] = hi; dst[p.M + e] = lo; dst[2 * p.M + e] = hi;
-                  }
-                }
-              } else if (kBf16) {
-                __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.out[0]) + off;
-                if (full4 && (p.ldo & 3) == 0) {
-                  uint2 pk;
-                  pk.x = pack_bf16(v[0], v[1]);
-                  pk.y = pack_bf16(v[2], v[3]);
-                  *reinterpret_cast<uint2*>(dst) = pk;
-                } else {
-                  for (int e = 0; e < 4; ++e)
-                    if (f0 + e < p.M) dst[e] = __float2bfloat16_rn(v[e]);
-                }
-              } else {
-                float* dst = reinterpret_cast<float*>(p.out[0]) + off;
-                if (full4 && (p.ldo & 3) == 0) {
-                  *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
-                } else if (full4 && (p.ldo & 1) == 0) {
-                  *reinterpret_cast<float2*>(dst) = make_float2(v[0], v[1]);
-                  *reinterpret_cast<float2*>(dst + 2) = make_float2(v[2], v[3]);
-                } else {
-                  for (int e = 0; e < 4; ++e)
-                    if (f0 + e < p.M) dst[e] = v[e];
-                }
-              }
+          for (int hh = 0; hh < 2; ++hh) {
+            const int r64 = warp * 16 + (lane >> 2) + 8 * hh;     // row within the warpgroup's 64
+            const int c64 = j8 * 8 + 2 * (lane & 3);              // column within the chunk (even)
+            const int r = r64 & 31, c = c64 & 31;
+            uint8_t* blk = stg_wg + ((c64 >> 5) * 2 + (r64 >> 5)) * (32 * 128);
+            const float v0 = acc[4 * (cc * 8 + j8) + 2 * hh], v1 = acc[4 * (cc * 8 + j8) + 2 * hh + 1];
+            if (!kTransposed) {
+              *reinterpret_cast<float2*>(blk + r * 128 + (((c >> 2) ^ (r & 7)) << 4) + (c & 3) * 4) = make_float2(v0, v1);
+            } else {
+              *reinterpret_cast<float*>(blk + c * 128 + (((r >> 2) ^ (c & 7)) << 4) + (r & 3) * 4) = v0;
+              *reinterpret_cast<float*>(blk + (c + 1) * 128 + (((r >> 2) ^ ((c + 1) & 7)) << 4) + (r & 3) * 4) = v1;
             }
           }
-          __syncwarp();
         }
+        named_bar_sync(1 + mw, 128);
+        const int n0 = n_blk * BN + cc * 64 + (warp >> 1) * 32;
+        if (!kTransposed) {
+          if (n0 < p.N) epi_store_normal<EPI>(p, stg, lane, n0, row0, ooff, okmask);
+        } else {
+          epi_store_transposed<EPI>(p, stg, lane, n0, row0, split, store_ok);
+        }
+        named_bar_sync(1 + mw, 128);   // the staging buffer is rewritten by the next chunk
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[accum]);
-      accum ^= 1;
-      if (accum == 0) accum_phase ^= 1;
     }
   }
 
-  tc_fence_before();
   __syncthreads();
   if (p.pdl) tl_mark(200000 + 1000 + static_cast<int>(gridDim.x));
   if (chained && threadIdx.x == 0) chain_signal_thread0(p.chain);
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, C::TMEM_COLS);
-  }
 }
 
 }  // namespace gitb200

@@ -1,4 +1,4 @@
-// libgitb200.so -- C ABI + host-side engine of the B200-native GIT captioning hot path.
+// libgitb200.so -- C ABI + host-side engine of the H100-native (sm_90a) GIT captioning hot path.
 // See include/gitb200.h for the contract of every entry point and the reference function it replaces.
 //
 // Device data layout (all engine-owned, HBM resident):
@@ -31,7 +31,6 @@
 #include "constrained.cuh"
 #include "decode_mega.cuh"
 #include "gemm.cuh"
-#include "gemm2.cuh"
 #include "preproc.cuh"
 #include "ptx.cuh"
 #include "rowops.cuh"
@@ -40,7 +39,7 @@
 using namespace gitb200;
 typedef __nv_bfloat16 bf16;
 
-#define GITB200_ABI_VERSION 5
+#define GITB200_ABI_VERSION 6
 
 // ------------------------------------------------------------------------------------------------
 // errors
@@ -105,20 +104,18 @@ struct TmapKey {
 struct gitb200_engine {
   gitb200_config cfg;
   int device = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   std::string err;
   int64_t launches = 0;
   bool use_graph = true;
   bool use_pdl = true;
   bool use_chain = true;
-  bool use_2cta = true;   // encoder / prefill GEMMs through the cta_group::2 kernel (gemm2.cuh)
   // fp32-grade parity mode: every GEMM operand is a (hi, lo) bf16 pair and each GEMM computes a_hi w_hi + a_lo w_hi +
-  // a_hi w_lo in ONE pass of the same tcgen05 kernel (activations stored [hi | lo | hi], weights [hi | hi | lo] along K);
+  // a_hi w_lo in ONE pass of the same wgmma kernel (activations stored [hi | lo | hi], weights [hi | hi | lo] along K);
   // attention, K/V caches and q/k/v stay fp32; exact QuickGELU.  ~3x the GEMM work: a verification mode (the north star's
   // "logits within 1e-3" against the fp32 reference), not a serving mode.  Weights must be (re-)uploaded after switching.
-  bool tc_attn = true;    // ViT / prefill attention on tcgen05 (flash_attn_tc_kernel) when the sequence fits TMEM (S <= 512)
   bool use_mega = true;   // greedy decode steps of <= 64 sequences through the persistent decode_mega_kernel
-  bool mega_coop = true;  // ... launched cooperatively (co-residency of its 148 CTAs guaranteed by the driver)
+  bool mega_coop = true;  // ... launched cooperatively (co-residency of its one-per-SM CTAs guaranteed by the driver)
   bool mega_ready = false;
   int debug_layers = -1;  // debugging: run only the first n decoder layers in the decode step (both step paths); -1 = all
   bool parity = false;
@@ -310,7 +307,7 @@ static int launch_gemm_inst(gitb200_engine* h, const GemmCall& c, cudaStream_t s
   using C = GemmCfg<BN>;
   static bool attr_set[64] = {false};
   if (!attr_set[h->device & 63]) {
-    CK(cudaFuncSetAttribute(gemm_bf16_tcgen05<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+    CK(cudaFuncSetAttribute(gemm_bf16_wgmma<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
     attr_set[h->device & 63] = true;
   }
   CUtensorMap ta, tb;
@@ -321,44 +318,9 @@ static int launch_gemm_inst(gitb200_engine* h, const GemmCall& c, cudaStream_t s
   const int tiles = m_tiles * n_tiles * c.p.k_splits;
   const int grid = tiles < h->num_sms ? tiles : h->num_sms;
   h->last_gemm_grid = grid;
-  CK(launch_k(c.p.pdl != 0, gemm_bf16_tcgen05<BN, EPI>, dim3(grid), dim3(C::THREADS), C::SMEM_BYTES, st, ta, tb, c.p));
-  CKL(h, "gemm_bf16_tcgen05");
+  CK(launch_k(c.p.pdl != 0, gemm_bf16_wgmma<BN, EPI>, dim3(grid), dim3(C::THREADS), C::SMEM_BYTES, st, ta, tb, c.p));
+  CKL(h, "gemm_bf16_wgmma");
   return 0;
-}
-
-template <int BN, int EPI>
-static int launch_gemm2_inst(gitb200_engine* h, const GemmCall& c, cudaStream_t st) {
-  using C = Gemm2Cfg<BN>;
-  static bool attr_set[64] = {false};
-  if (!attr_set[h->device & 63]) {
-    CK(cudaFuncSetAttribute(gemm2_bf16_tcgen05<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
-    attr_set[h->device & 63] = true;
-  }
-  CUtensorMap ta, tb;
-  TRY(get_tmap(h, c.A, c.p.M, c.p.K, c.lda, 128, &ta));
-  TRY(get_tmap(h, c.B, c.p.N, c.p.K, c.ldb, BN / 2, &tb));
-  const int m_tiles = (c.p.M + 255) / 256;
-  const int n_tiles = (c.p.N + BN - 1) / BN;
-  const int tiles = m_tiles * n_tiles;
-  const int pairs = std::min(tiles, h->num_sms / 2);
-  h->last_gemm_grid = 2 * pairs;
-  CK(launch_k(false, gemm2_bf16_tcgen05<BN, EPI>, dim3(2 * pairs), dim3(C::THREADS), C::SMEM_BYTES, st, ta, tb, c.p));
-  CKL(h, "gemm2_bf16_tcgen05");
-  return 0;
-}
-// The epilogue variants the hot path uses (each is its own kernel instantiation).
-template <int BN>
-static int launch_gemm2_bn(gitb200_engine* h, const GemmCall& c, cudaStream_t st) {
-  const GemmParams& p = c.p;
-  switch (epi_code(false, p.out_bf16 != 0, p.resid != nullptr, false, p.act)) {
-    case epi_code(false, true, false, false, ACT_NONE): return launch_gemm2_inst<BN, epi_code(false, true, false, false, ACT_NONE)>(h, c, st);
-    case epi_code(false, false, true, false, ACT_NONE): return launch_gemm2_inst<BN, epi_code(false, false, true, false, ACT_NONE)>(h, c, st);
-    case epi_code(false, false, false, false, ACT_NONE): return launch_gemm2_inst<BN, epi_code(false, false, false, false, ACT_NONE)>(h, c, st);
-    case epi_code(false, true, false, false, ACT_QUICKGELU): return launch_gemm2_inst<BN, epi_code(false, true, false, false, ACT_QUICKGELU)>(h, c, st);
-    case epi_code(false, true, false, false, ACT_GELU_ERF): return launch_gemm2_inst<BN, epi_code(false, true, false, false, ACT_GELU_ERF)>(h, c, st);
-    default: break;
-  }
-  return fail(h, "gemm2: epilogue combination not instantiated");
 }
 
 template <int BN>
@@ -400,9 +362,8 @@ static int launch_gemm_bn(gitb200_engine* h, const GemmCall& c, cudaStream_t st)
 
 static int pick_bn(const gitb200_engine* h, int M, int N, bool transposed) {
   if (transposed) return N <= 64 ? 64 : (N <= 128 ? 128 : 256);
-  // Measured on B200 (tools/gemm_sweep.py, M = 12608): wide outputs (N = 2304 / 3072) run best with 128x256 tiles
-  // (fewest operand bytes per FLOP through L2/shared memory); N = 768 with 128x192 tiles (4 column tiles: less
-  // wave quantisation than 3 x 256 at 99 row tiles over 148 SMs).
+  // Wide outputs (N = 2304 / 3072) take 128x256 tiles (fewest operand bytes per FLOP through L2 / shared memory); N = 768
+  // takes 128x192 tiles (4 column tiles: less wave quantisation than 3 x 256 at 99 row tiles over 132 SMs).
   (void)h; (void)M;
   if (N % 256 == 0 && N >= 1024) return 256;
   if (N % 192 == 0) return 192;
@@ -432,21 +393,6 @@ static int launch_gemm(gitb200_engine* h, GemmCall c, cudaStream_t st) {
   if (p.partial && p.split_stride < static_cast<long long>(p.N) * p.ldo) return fail(h, "gemm: split_stride smaller than one partial buffer");
   int bn = c.bn > 0 ? c.bn : pick_bn(h, p.M, p.N, p.transposed != 0);
   if (p.split3 && !p.transposed) bn = 256;
-  // 2-CTA (cta_group::2) kernel: explicit request (bn = 1000 + BN, unit tests) or engine option for the big GEMMs
-  // Measured (tools/gemm_sweep.py, M = 12608): pairs win on wide outputs (+7-10 %) and on K = 3072 (+11 %); the
-  // K = N = 768 out-projection is epilogue bound and stays on 1-CTA 128x192 tiles.
-  if (bn < 1000 && h->use_2cta && !h->parity && !p.transposed && p.k_splits == 1 && p.M >= 2048) {
-    if (p.N % 256 == 0 && p.N >= 1024) bn = 1256;
-    else if (p.N % 192 == 0 && p.K >= 1536) bn = 1192;
-  }
-  if (bn >= 1000) {
-    if (p.transposed || p.k_splits != 1) return fail(h, "gemm2: normal epilogue, no split-K");
-    switch (bn - 1000) {
-      case 256: return launch_gemm2_bn<256>(h, c, st);
-      case 192: return launch_gemm2_bn<192>(h, c, st);
-      default: return fail(h, "gemm2: unsupported tile width %d", bn - 1000);
-    }
-  }
   switch (bn) {
     case 64: return launch_gemm_bn<64>(h, c, st);
     case 128: return launch_gemm_bn<128>(h, c, st);
@@ -509,66 +455,25 @@ static void launch_flash(const AttnParams& p, cudaStream_t st) {
   dim3 grid((p.S + NW * 16 - 1) / (NW * 16), p.H, p.B);
   flash_attn_kernel<NW><<<grid, NW * 32, 0, st>>>(p);
 }
-// tcgen05 attention (attention.cuh: flash_attn_tc_kernel) for sequences whose scores fit the tensor memory in one piece
-static int launch_attention_tc(gitb200_engine* h, const AttnParams& ap, cudaStream_t st) {
-  AttnTcParams p{};
-  p.out = ap.out; p.B = ap.B; p.S = ap.S; p.H = ap.H;
-  p.spad = (ap.S + 15) / 16 * 16;
-  if (p.spad <= 256) { p.kv_boxes = 1; p.kv_box_rows = p.spad; }
-  else { p.kv_boxes = 2; p.kv_box_rows = ((p.spad + 1) / 2 + 7) / 8 * 8; }
-  p.q_rows_per_batch = ap.S; p.kv_rows_per_batch = ap.S;
-  p.q_col0 = 0; p.k_col0 = 0; p.v_col0 = 0;
-  p.o_rs = ap.o_rs; p.o_bs = ap.o_bs;
+// Hopper attention (attention.cuh: flash_attn_wgmma_kernel) for batches stored back to back (row b * S + i of the q / k / v
+// views), which is every ViT and prefill call; TMA needs the row pitch and the bases 16-byte aligned (get_tmap checks).
+static int launch_attention_wgmma(gitb200_engine* h, const AttnParams& ap, cudaStream_t st) {
+  AttnParams p = ap;
   p.scale_log2 = 0.125f * 1.44269504088896340736f;
   const long long rows = static_cast<long long>(ap.B) * ap.S;
   CUtensorMap tq, tk, tv;
-  TRY(get_tmap(h, ap.q, rows, ap.H * 64, ap.q_rs, 128, &tq));
-  TRY(get_tmap(h, ap.k, rows, ap.H * 64, ap.kv_rs, p.kv_box_rows, &tk));
-  TRY(get_tmap(h, ap.v, rows, ap.H * 64, ap.kv_rs, p.kv_box_rows, &tv));
-  const size_t smem = attn_tc_smem_bytes(p.spad, p.kv_box_rows, p.kv_boxes);
-  static size_t attr_done[64] = {0};
-  if (attr_done[h->device & 63] < smem) {
-    CK(cudaFuncSetAttribute(flash_attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    attr_done[h->device & 63] = smem;
-  }
-  flash_attn_tc_kernel<<<dim3(ap.H, ap.B), kAttnTcThreads, smem, st>>>(tq, tk, tv, p);
-  CKL(h, "flash_attn_tc_kernel");
-  return 0;
-}
-
-// tcgen05 attention for sequences beyond the tensor memory (attention.cuh: flash_attn_tc_long_kernel): 128-key blocks, two passes
-static int launch_attention_tc_long(gitb200_engine* h, const AttnParams& ap, cudaStream_t st) {
-  AttnTcParams p{};
-  p.out = ap.out; p.B = ap.B; p.S = ap.S; p.H = ap.H;
-  p.spad = (ap.S + 15) / 16 * 16;
-  p.kv_boxes = 1; p.kv_box_rows = kAttnLongBlk;
-  p.q_rows_per_batch = ap.S; p.kv_rows_per_batch = ap.S;
-  p.q_col0 = 0; p.k_col0 = 0; p.v_col0 = 0;
-  p.o_rs = ap.o_rs; p.o_bs = ap.o_bs;
-  p.scale_log2 = 0.125f * 1.44269504088896340736f;
-  const long long rows = static_cast<long long>(ap.B) * ap.S;
-  CUtensorMap tq, tk, tv;
-  TRY(get_tmap(h, ap.q, rows, ap.H * 64, ap.q_rs, 128, &tq));
-  TRY(get_tmap(h, ap.k, rows, ap.H * 64, ap.kv_rs, kAttnLongBlk, &tk));
-  TRY(get_tmap(h, ap.v, rows, ap.H * 64, ap.kv_rs, kAttnLongBlk, &tv));
-  const size_t smem = attn_tc_long_smem_bytes();
-  static bool attr_done[64] = {false};
-  if (!attr_done[h->device & 63]) {
-    CK(cudaFuncSetAttribute(flash_attn_tc_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    attr_done[h->device & 63] = true;
-  }
-  flash_attn_tc_long_kernel<<<dim3(ap.H, ap.B, (ap.S + 127) / 128), kAttnTcThreads, smem, st>>>(tq, tk, tv, p);
-  CKL(h, "flash_attn_tc_long_kernel");
+  TRY(get_tmap(h, ap.q, rows, ap.H * 64, ap.q_rs, kAttnWgRows, &tq));
+  TRY(get_tmap(h, ap.k, rows, ap.H * 64, ap.kv_rs, kAttnWgRows, &tk));
+  TRY(get_tmap(h, ap.v, rows, ap.H * 64, ap.kv_rs, kAttnWgRows, &tv));
+  flash_attn_wgmma_kernel<<<dim3((ap.S + kAttnWgRows - 1) / kAttnWgRows, ap.H, ap.B), 128, kAttnWgSmem, st>>>(tq, tk, tv, p);
+  CKL(h, "flash_attn_wgmma_kernel");
   return 0;
 }
 
 static int launch_attention(gitb200_engine* h, const AttnParams& ap, cudaStream_t st) {
-  if (h->tc_attn && ap.S <= 512 && ap.q_bs == static_cast<long long>(ap.S) * ap.q_rs && ap.kv_bs == static_cast<long long>(ap.S) * ap.kv_rs &&
-      attn_tc_smem_bytes((ap.S + 15) / 16 * 16, ap.S <= 256 ? (ap.S + 15) / 16 * 16 : (((ap.S + 15) / 16 * 16 + 1) / 2 + 7) / 8 * 8,
-                         ap.S <= 256 ? 1 : 2) <= 226 * 1024)
-    return launch_attention_tc(h, ap, st);
-  if (h->tc_attn && ap.S > 512 && ap.q_bs == static_cast<long long>(ap.S) * ap.q_rs && ap.kv_bs == static_cast<long long>(ap.S) * ap.kv_rs)
-    return launch_attention_tc_long(h, ap, st);
+  if (ap.q_bs == static_cast<long long>(ap.S) * ap.q_rs && ap.kv_bs == static_cast<long long>(ap.S) * ap.kv_rs)
+    return launch_attention_wgmma(h, ap, st);
+  // flash_attn_kernel: batches with other strides
   AttnParams p = ap;
   p.scale_log2 = 0.125f * 1.44269504088896340736f;
   // query rows per CTA = 16 * NW: least padding first, then the larger tile (K/V are re-read per query tile)
@@ -671,9 +576,7 @@ extern "C" int gitb200_set_option(gitb200_engine* h, const char* name, int64_t v
   if (strcmp(name, "use_graph") == 0) { h->use_graph = value != 0; return 0; }
   if (strcmp(name, "use_pdl") == 0) { h->use_pdl = value != 0; return 0; }
   if (strcmp(name, "use_chain") == 0) { h->use_chain = value != 0; return 0; }
-  if (strcmp(name, "use_2cta") == 0) { h->use_2cta = value != 0; return 0; }
   if (strcmp(name, "use_mega") == 0) { h->use_mega = value != 0; return 0; }
-  if (strcmp(name, "tc_attn") == 0) { h->tc_attn = value != 0; return 0; }
   if (strcmp(name, "debug_layers") == 0) { h->debug_layers = static_cast<int>(value); return 0; }
   if (strcmp(name, "mega_coop") == 0) { h->mega_coop = value != 0; return 0; }
   if (strcmp(name, "parity") == 0) {
@@ -708,8 +611,8 @@ extern "C" int gitb200_create(const gitb200_config* cfg, int device, gitb200_eng
   if (device < 0 || device >= ndev) return fail(nullptr, "gitb200_create: bad device %d", device);
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return fail(nullptr, "cudaGetDeviceProperties failed");
-  if (prop.major != 10)
-    return fail(nullptr, "gitb200_create: device %d is sm_%d%d; this library contains sm_100a code only", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(nullptr, "gitb200_create: device %d is sm_%d%d; this library contains sm_90a code only", device, prop.major, prop.minor);
   if (cfg->image_size % cfg->patch != 0) return fail(nullptr, "image_size %% patch != 0");
   if (cfg->enc_width != 768 && cfg->enc_width != 1024) return fail(nullptr, "enc_width must be 768 or 1024");
   if (cfg->dec_hidden != 768 || cfg->dec_heads * 64 != cfg->dec_hidden || cfg->enc_heads * 64 != cfg->enc_width)
@@ -816,7 +719,7 @@ static int store_bf16(gitb200_engine* h, DevBuf& dst, long long total_rows, long
                       const float* src, long long rows, long long cols, cudaStream_t st) {
   CK(dst.ensure(static_cast<size_t>(total_rows) * dst_cols * h->ks() * sizeof(bf16)));
   const long long total = rows * dst_cols;
-  const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, 148 * 16));
+  const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, static_cast<long long>(h->num_sms) * 16));
   if (h->parity) cvt_rows_split3_kernel<<<grid, 256, 0, st>>>(src, cols, dst.as<bf16>() + row_off * 3 * dst_cols, rows, cols, dst_cols);
   else cvt_rows_kernel<<<grid, 256, 0, st>>>(src, cols, dst.as<bf16>() + row_off * dst_cols, dst_cols, rows, cols, dst_cols);
   CKL(h, "cvt_rows_kernel");
@@ -965,7 +868,7 @@ extern "C" int gitb200_finalize_weights(gitb200_engine* h, void* stream) {
     auto pack = [&](DevBuf& dst, const DevBuf& src, long long ldw, int n_feat, int k0, long long n_tiles, int stride, int offset) -> int {
       CK(dst.ensure(static_cast<size_t>(n_tiles) * stride * kMegaTileBytes));
       const long long total = n_tiles * 48 * 32;
-      pack_tiles_kernel<<<static_cast<int>(std::min<long long>((total + 255) / 256, 148 * 16)), 256, 0, st>>>(
+      pack_tiles_kernel<<<static_cast<int>(std::min<long long>((total + 255) / 256, static_cast<long long>(h->num_sms) * 16)), 256, 0, st>>>(
           src.as<bf16>(), ldw, n_feat, k0, dst.as<uint8_t>(), n_tiles, stride, offset);
       CKL(h, "pack_tiles_kernel");
       return 0;
@@ -1322,7 +1225,7 @@ static int step_layers(gitb200_engine* h, Lane& ln_, const long long* tokens, co
 static int set_attn_smem_limit(gitb200_engine* h) {
   const int M = h->cur_M;
   // chunks of at most 224 keys: two (K + V) staging buffers of one chunk per CTA, and at least two CTAs per SM (M = 257
-  // in one piece was 131 KB per CTA = one 4-warp CTA per SM: 44 us per launch at 128 beam rows, profiles/launches_r02_config3.csv)
+  // in one piece would be 131 KB per CTA = one 4-warp CTA per SM)
   const int n_chunks = (M + 223) / 224;
   h->attn_box_rows = (M + n_chunks - 1) / n_chunks;
   h->attn_chunk_rows = h->attn_box_rows;

@@ -69,8 +69,8 @@ __device__ __forceinline__ float beam_length_norm(int length, float lp) {
 }
 
 // Sorted candidate list of kMaxCand entries in registers (descending value, ascending index on exact ties).  Every access is
-// statically indexed: the round-1 version indexed the arrays with a runtime position, which put them in local memory and
-// made this kernel 144 us per step at 128 rows (profiles/launches_r02_config3.csv).
+// statically indexed: indexing the arrays with a runtime position puts them in local memory, which made this kernel
+// several times slower.
 struct TopList {
   float v[kMaxCand];
   int i[kMaxCand];

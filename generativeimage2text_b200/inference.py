@@ -149,7 +149,7 @@ class ImageTransform(object):
     # -- pixels (GPU) ------------------------------------------------------------------------------------------
     def _ensure(self):
         if self.device is None or self.device.type != 'cuda':
-            raise RuntimeError('the image transform runs on CUDA devices only (libgitb200.so, sm_100a); there is no CPU path')
+            raise RuntimeError('the image transform runs on CUDA devices only (libgitb200.so, sm_90a); there is no CPU path')
         if self._handle is None:
             h = ctypes.c_void_p()
             lib = _lib.load()

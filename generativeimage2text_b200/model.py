@@ -5,7 +5,7 @@ The returned `torch.nn.Module` carries parameters under the reference's own stat
 `torch_common.load_state_dict`, reference torch_common.py:93-145, and `.cuda()/.eval()` work unchanged) and
 its `forward(batch)` accepts the reference's batch dict and returns `{'predictions', 'logprobs'}`
 (reference layers/decoder.py:838-877, 977-1011) -- but no PyTorch op touches the hot path: pixels go in,
-token ids come out of libgitb200.so (hand-written sm_100a kernels).  PyTorch only owns the parameter
+token ids come out of libgitb200.so (hand-written sm_90a kernels).  PyTorch only owns the parameter
 storage, the CUDA stream and the output tensors.
 """
 import ctypes
@@ -322,7 +322,7 @@ class GitB200CaptioningModel(nn.Module):
     def _ensure_engine(self, slot=0):
         dev = self._device()
         if dev.type != 'cuda':
-            raise RuntimeError('the gitb200 engine runs on CUDA devices only (sm_100a); call model.cuda() first. '
+            raise RuntimeError('the gitb200 engine runs on CUDA devices only (sm_90a); call model.cuda() first. '
                                'There is no CPU path.')
         lib = _lib.load()
         if self._engine_device is not None and self._engine_device != dev:
@@ -335,8 +335,8 @@ class GitB200CaptioningModel(nn.Module):
             _lib.check(lib.gitb200_create(ctypes.byref(self._cfg), dev.index or 0, ctypes.byref(h)), None, 'create')
             sl['engine'], sl['sig'], sl['trie_key'] = h, None, None
             import os
-            for opt in ('use_graph', 'use_pdl', 'use_chain', 'use_2cta', 'use_mega', 'mega_coop', 'tc_attn', 'debug_layers', 'parity'):
-                v = os.environ.get('GITB200_' + opt.upper())      # debugging switches, e.g. GITB200_USE_2CTA=0
+            for opt in ('use_graph', 'use_pdl', 'use_chain', 'use_mega', 'mega_coop', 'debug_layers', 'parity'):
+                v = os.environ.get('GITB200_' + opt.upper())      # debugging switches, e.g. GITB200_USE_MEGA=0
                 if v is not None:
                     _lib.check(lib.gitb200_set_option(h, opt.encode(), int(v)), h, 'set_option')
             for opt, v in self._options.items():                  # set_engine_option() calls made so far
@@ -381,9 +381,9 @@ class GitB200CaptioningModel(nn.Module):
             pass
 
     def set_engine_option(self, name, value):
-        """Engine switches (0/1): 'use_graph', 'use_pdl', 'use_chain', 'use_2cta', 'use_mega' (persistent one-kernel decode
+        """Engine switches (0/1): 'use_graph', 'use_pdl', 'use_chain', 'use_mega' (persistent one-kernel decode
         step for greedy batches of <= 64), and 'parity' -- the fp32-grade
-        verification mode (every GEMM as a three-term bf16 split product through the same tcgen05 kernels, fp32
+        verification mode (every GEMM as a three-term bf16 split product through the same wgmma kernels, fp32
         attention and K/V caches): logits within 1e-3 of the fp32 reference at ~3x the GEMM work."""
         self._options[name] = int(value)
         if name == 'parity':
@@ -600,7 +600,7 @@ class GitB200CaptioningModel(nn.Module):
     def _submit_coalesced(self, image, depth, want):
         dev = self._device()
         if dev.type != 'cuda':
-            raise RuntimeError('the gitb200 engine runs on CUDA devices only (sm_100a); call model.cuda() first. '
+            raise RuntimeError('the gitb200 engine runs on CUDA devices only (sm_90a); call model.cuda() first. '
                                'There is no CPU path.')
 
         def to_dev(t):

@@ -164,7 +164,7 @@ def synthetic_state_dict(param=None, seed=0, variant='init'):
 
 
 DECISIVE_LIVE = 8      # tokens that stay in play in the 'decisive' variant (EOS is one of them)
-# decoder attention sharpening of the 'decisive' variant (q, k weights / attention output weights).  Chosen on B200 with
+# decoder attention sharpening of the 'decisive' variant (q, k weights / attention output weights).  Chosen with
 # tools/decisive_pick.py: the sharper the softmax the more the captions depend on the image -- and the more bf16 rounding is
 # amplified; x8 / x4 made the decoder chaotic (12.5 max logit error), these values keep the error at the random-init level
 DECISIVE_QK_SCALE = 2.0

@@ -1,9 +1,9 @@
-/* gitb200 -- C ABI of the B200-native GIT captioning engine (libgitb200.so).
+/* gitb200 -- C ABI of the H100-native (sm_90a) GIT captioning engine (libgitb200.so).
  *
  * This is the drop-in boundary for the reference's hot path.  The reference is 100 % Python/PyTorch
  * (there is no FFI of its own), so the "binding a maintainer would add" is a ctypes stub
  * (INTEGRATION.md); each entry point names the reference function it replaces.  Paths are relative to
- * /root/reference/generativeimage2text/.
+ * the reference's generativeimage2text/.
  *
  * Conventions
  *   - plain C types only; every `dev` pointer is a CUDA device pointer owned by the caller
@@ -174,10 +174,10 @@ int gitb200_set_sampling(gitb200_engine* h, const float* uniforms_dev, int steps
 /* Number of kernels the engine launched since creation (bench.py's gpu_launches). */
 int64_t gitb200_launch_count(const gitb200_engine* h);
 /* Engine switches (defaults in parentheses): use_graph (1) CUDA-graph replay of the decode step, use_pdl (1) programmatic
- * dependent launch inside the step, use_chain (1) flag-ordered decode chain, use_2cta (1) cta_group::2 encoder GEMMs,
+ * dependent launch inside the step, use_chain (1) flag-ordered decode chain,
  * use_mega (1) greedy decode steps of <= 64 sequences as one persistent kernel (mega_coop (1): launched cooperatively),
  * parity (0) fp32-grade verification mode: every GEMM operand is a (hi, lo) bf16 pair and each product is computed as
- * a_hi w_hi + a_lo w_hi + a_hi w_lo by the same tcgen05 kernel (three K-segments side by side), attention / K/V caches /
+ * a_hi w_hi + a_lo w_hi + a_hi w_lo by the same wgmma kernel (three K-segments side by side), attention / K/V caches /
  * q, k, v in fp32 -- set it BEFORE gitb200_set_weight (switching it forgets the uploaded weights). */
 int gitb200_set_option(gitb200_engine* h, const char* name, int64_t value);
 

@@ -3,13 +3,14 @@ captioning hot path.  It is the *checker* for the CUDA engine and the `cpu_basel
 bench.py; the product package never imports it (the product fails loudly without its CUDA library).
 
 Parity status: the reference ships no tests or golden vectors (SURVEY.md section 4), so this
-restatement is pinned against the reference's own modules executed in the build container:
-  * tests/test_oracle_vs_reference.py runs both on the same seeded weights/pixels (needs /root/reference);
+restatement is pinned against what the reference's own modules return:
+  * tests/test_oracle_vs_reference.py compares it with the reference's outputs on the same seeded weights/pixels
+    (tests/golden/reference_checks.json, oracle/make_reference_golden.py);
   * tests/golden/*.npz were produced by the *unmodified reference* (oracle/make_golden.py) and are
     checked against this file on every machine (tests/test_oracle_golden.py).
 
 Every function cites the reference file:line it follows (paths relative to
-/root/reference/generativeimage2text/).  Two execution modes of the decoder:
+the reference's generativeimage2text/).  Two execution modes of the decoder:
   * `CachedDecoder`   -- KV-cached single-row steps (results-equivalent, SURVEY.md Appendix A
                          "KV-cache equivalence"); used for checking, it is what the engine implements.
   * `as_shipped_step` -- recomputes the whole [image || text] sequence every step exactly like the

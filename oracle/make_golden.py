@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY -- generates tests/golden/*.npz by running the UNMODIFIED reference
-(/root/reference, imported through oracle/ref_shim.py) on seeded synthetic checkpoints.
+(imported through oracle/ref_shim.py) on seeded synthetic checkpoints.
 
-Run in the build container only:  python oracle/make_golden.py [case ...]
+Run where the reference is importable:  python oracle/make_golden.py [case ...]
 
 The reference ships no golden vectors of its own (SURVEY.md section 4); these fixtures pin
 oracle/git_oracle.py (tests/test_oracle_golden.py) and, through it and directly, the CUDA engine.

@@ -1,9 +1,8 @@
-"""TEST INFRASTRUCTURE ONLY -- imports the *unmodified* reference from /root/reference.
+"""TEST INFRASTRUCTURE ONLY -- imports the *unmodified* reference (a microsoft/GenerativeImage2Text checkout at
+$GIT_REFERENCE_ROOT, default ../GenerativeImage2Text next to this repository).
 
-Only usable in the build container (the GPU box has no /root/reference); it is used
-by oracle/make_golden.py to generate tests/golden/* and by
-tests/test_oracle_vs_reference.py to pin oracle/git_oracle.py against the reference's
-own modules.  Nothing in the product package may import this file.
+Used by oracle/make_golden.py and oracle/make_reference_golden.py to generate tests/golden/*; the tests themselves only
+read those files.  Nothing in the product package may import this file.
 
 Shims (SURVEY.md section 8c / Appendix B):
   * `azfuse`, `boto3`, `botocore` are absent -> stub packages in oracle/stubs
@@ -19,7 +18,8 @@ import sys
 
 import torch
 
-REFERENCE_ROOT = os.environ.get('GIT_REFERENCE_ROOT', '/root/reference')
+REFERENCE_ROOT = os.environ.get('GIT_REFERENCE_ROOT', os.path.join(os.path.dirname(os.path.dirname(os.path.dirname(
+    os.path.abspath(__file__)))), 'GenerativeImage2Text'))
 _STUBS = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'stubs')
 
 CLIP_CFG = {

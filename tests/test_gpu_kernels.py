@@ -53,7 +53,7 @@ def _rand(shape, scale=1.0, seed=0, dtype=torch.bfloat16):
     (128, 128, 256, 128),     # accumulate over k-blocks inside one swizzle ring
     (256, 256, 1024, 128),    # pipeline wrap-around (16 k-blocks > stages)
     (1000, 768, 768, 128), (1000, 768, 768, 192), (1000, 768, 768, 256),
-    (12608, 768, 768, 0),     # persistent: several tiles per CTA, TMEM double buffering, tail rows
+    (12608, 768, 768, 0),     # persistent: several tiles per CTA, tail rows
     (300, 3072, 776, 256),    # K tail (776 = 12*64 + 8) relies on TMA zero fill
 ])
 def test_gemm_plain(M, N, K, bn):
@@ -65,14 +65,14 @@ def test_gemm_plain(M, N, K, bn):
 
 
 @pytest.mark.parametrize('M,N,K,bn,act,out_bf16,use_resid', [
-    (256, 256, 64, 1256, 0, False, False),     # one pair, one tile, one k-block
-    (512, 512, 512, 1256, 0, True, False),     # several tiles, ring wrap-around
-    (1000, 768, 768, 1192, 0, False, True),    # M tail, 192-wide tiles, residual epilogue
-    (12608, 3072, 768, 1256, 1, True, False),  # ViT c_fc: persistent pairs, TMEM double buffering
-    (12608, 768, 3072, 1192, 0, False, True),  # ViT c_proj
+    (256, 256, 64, 256, 0, False, False),      # one tile, one k-block
+    (512, 512, 512, 256, 0, True, False),      # several tiles, ring wrap-around
+    (1000, 768, 768, 192, 0, False, True),     # M tail, 192-wide tiles, residual epilogue
+    (12608, 3072, 768, 256, 1, True, False),   # ViT c_fc: persistent CTAs, several tiles each
+    (12608, 768, 3072, 192, 0, False, True),   # ViT c_proj
 ])
-def test_gemm_2cta(M, N, K, bn, act, out_bf16, use_resid):
-    """cta_group::2 kernel (gemm2.cuh): CTA pairs computing 256 x BN tiles."""
+def test_gemm_wide_tiles(M, N, K, bn, act, out_bf16, use_resid):
+    """128 x 256 / 128 x 192 tiles at the encoder's GEMM shapes, with the epilogues those GEMMs use."""
     a, w = _rand((M, K), 1.0, 41), _rand((N, K), 0.05, 42)
     bias = _rand((N,), 0.5, 43, torch.float32)
     resid = _rand((M, N), 1.0, 44, torch.float32) if use_resid else None

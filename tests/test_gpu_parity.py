@@ -566,7 +566,7 @@ def _parity_model(meta, sd, **kw):
 @pytest.mark.parametrize('name', ['base_greedy_init', 'base_greedy', 'base_prefix', 'vatex_greedy', 'large_greedy',
                                   'base_ratio_greedy', 'base_decisive'])
 def test_parity_mode_logits_within_1e3_of_the_fp32_reference(name):
-    """Every GEMM as a three-term (hi, lo) bf16 split product through the same tcgen05 kernels, fp32 attention and caches:
+    """Every GEMM as a three-term (hi, lo) bf16 split product through the same wgmma kernels, fp32 attention and caches:
     image features, visual projection and every step's full logit row within 1e-3 of the fp32 oracle (and of the
     reference's own numbers at the golden's sampled columns), teacher-forced; decisions equal wherever the margin exceeds
     2.5x the measured error; and the FREE-RUNNING captions equal the reference's whenever every margin along the way does."""

@@ -8,7 +8,7 @@ import pytest
 import torch
 
 import preprocess_oracle as po
-import ref_shim
+from golden_io import load_reference_checks
 from generativeimage2text_b200 import inference as inf
 from generativeimage2text_b200 import _lib
 
@@ -32,15 +32,13 @@ def test_geometry_equals_oracle_rules(param):
             assert (oh, ow) == (crop, crop)
 
 
-@pytest.mark.skipif(not ref_shim.reference_available(), reason='no /root/reference')
 def test_minmax_equals_reference_class():
-    ref_shim._import_reference()
-    import generativeimage2text.inference as rinf
+    gold = load_reference_checks()['minmax_resize']
     for mn, mx in [(480, 640), (420, 560), (224, 224)]:
-        a, b = rinf.MinMaxResizeForTest(mn, mx), inf.MinMaxResizeForTest(mn, mx)
-        for h, w in SHAPES:
-            assert a.get_size((w, h)) == b.get_size((w, h))
-        assert repr(a) == repr(b)
+        b = inf.MinMaxResizeForTest(mn, mx)
+        want = gold['%d_%d' % (mn, mx)]
+        assert [list(b.get_size((w, h))) for h, w in SHAPES] == want['sizes']
+        assert repr(b) == want['repr']
 
 
 @pytest.mark.parametrize('pair', [(640, 298), (480, 224), (75, 224), (500, 720), (1920, 398), (3, 2), (5, 7), (224, 112),

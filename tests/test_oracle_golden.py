@@ -1,5 +1,5 @@
 """CPU: oracle/git_oracle.py against the golden vectors produced by the unmodified reference
-(oracle/make_golden.py).  This is what pins the oracle on machines without /root/reference."""
+(oracle/make_golden.py).  This is what pins the oracle without the original code at hand."""
 import numpy as np
 import pytest
 import torch

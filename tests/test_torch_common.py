@@ -1,11 +1,11 @@
-"""Checkpoint ingestion (SURVEY.md section 8f-1): generativeimage2text_b200/torch_common.py against the reference's
-torch_common.py (run here when /root/reference is present) and against hand-checked cases everywhere."""
+"""Checkpoint ingestion (SURVEY.md section 8f-1): generativeimage2text_b200/torch_common.py against what the original
+torch_common.py computes (tests/golden/reference_checks.json) and against hand-checked cases."""
 import collections
 
 import pytest
 import torch
 
-import ref_shim
+from golden_io import digest, load_reference_checks
 from generativeimage2text_b200 import torch_common as tc
 from generativeimage2text_b200.model import get_git_model
 from generativeimage2text_b200.synthetic import synthetic_state_dict
@@ -60,35 +60,27 @@ def test_load_state_dict_into_engine_shell(param):
     assert after['textual.output.weight'].data_ptr() == after['textual.embedding.words.weight'].data_ptr()
 
 
-@pytest.mark.skipif(not ref_shim.reference_available(), reason='no /root/reference')
 def test_same_result_as_reference_loader():
-    ref_shim._import_reference()
-    import generativeimage2text.torch_common as rtc
+    """The original torch_common.load_state_dict on the same messy checkpoint (stored digests of every resulting tensor)."""
+    gold = load_reference_checks()['loader']
     param = {'num_image_with_embedding': 6}
     ckpt, _ = _messy_checkpoint(param)
-    ref = ref_shim.load_reference_model(param, 'stock')
     ours = get_git_model(Tok(), param)
     # same starting point for the tensors the checkpoint does not provide
-    start = synthetic_state_dict(param, 11, 'init')
-    ref.load_state_dict(start, strict=False)
-    ours.load_state_dict(start, strict=True)
-    rtc.load_state_dict(ref, ckpt)
+    ours.load_state_dict(synthetic_state_dict(param, 11, 'init'), strict=True)
     tc.load_state_dict(ours, ckpt)
-    rsd, osd = ref.state_dict(), ours.state_dict()
-    assert list(rsd.keys()) == list(osd.keys())
-    for k in rsd:
-        assert torch.equal(rsd[k], osd[k]), k
+    osd = ours.state_dict()
+    assert list(osd.keys()) == gold['keys']
+    for k, want in zip(gold['keys'], gold['digests']):
+        assert digest(osd[k]) == want, k
 
 
-@pytest.mark.skipif(not ref_shim.reference_available(), reason='no /root/reference')
 @pytest.mark.parametrize('patch,width,after', [(16, 768, 480), (14, 1024, 420), (16, 768, 160)])
 def test_resize_2d_pos_embed_equals_reference(patch, width, after):
-    ref_shim._import_reference()
-    import generativeimage2text.torch_common as rtc
+    gold = load_reference_checks()['resize_2d_pos_embed']['%d_%d_%d' % (patch, width, after)]
     g = 224 // patch
     pe = torch.randn(g * g + 1, width, generator=torch.Generator().manual_seed(5))
-    a = rtc.resize_2d_pos_embed(pe, 224, patch, after)
     b = tc.resize_2d_pos_embed(pe, 224, patch, after)
-    assert a.shape == b.shape == ((after // patch) ** 2 + 1, width)
-    assert torch.equal(a, b)
-    assert torch.equal(rtc.resize_2d_pos_embed(pe[None], 224, patch, after), tc.resize_2d_pos_embed(pe[None], 224, patch, after))
+    assert list(b.shape) == gold['shape'] == [(after // patch) ** 2 + 1, width]
+    assert digest(b) == gold['digest']
+    assert digest(tc.resize_2d_pos_embed(pe[None], 224, patch, after)) == gold['digest_batched']

@@ -1,5 +1,5 @@
-"""TSV container I/O (SURVEY.md section 8f-3): generativeimage2text_b200/tsv_io.py -- format checks everywhere, and
-byte-for-byte against the reference's tsv_io.py when /root/reference is present."""
+"""TSV container I/O (SURVEY.md section 8f-3): generativeimage2text_b200/tsv_io.py -- format checks, and byte-for-byte
+against what the original tsv_io.py writes (tests/golden/reference_checks.json)."""
 import base64
 import json
 import os
@@ -7,7 +7,7 @@ import os
 import numpy as np
 import pytest
 
-import ref_shim
+from golden_io import file_digest, load_reference_checks
 from generativeimage2text_b200 import tsv_io
 
 
@@ -87,34 +87,23 @@ def test_concat_parts(tmp_path):
         assert t[i][0] == allrows[i][0] and t[i][1].encode() == allrows[i][1]
 
 
-@pytest.mark.skipif(not ref_shim.reference_available(), reason='no /root/reference')
 def test_byte_identical_to_reference_tsv_io(tmp_path):
-    ref_shim._import_reference()
-    import generativeimage2text.tsv_io as rio
+    """The files the original tsv_io.py writes for the same rows, and what its reader returns (stored digests)."""
+    gold = load_reference_checks()['tsv']
     rows = _rows(23, 7)
-    a, b = str(tmp_path / 'ours.tsv'), str(tmp_path / 'ref.tsv')
+    a = str(tmp_path / 'ours.tsv')
     tsv_io.tsv_writer(iter(rows), a)
-    rio.tsv_writer(iter(rows), b)
-    for fa, fb in zip(_files(a), _files(b)):
-        assert open(fa, 'rb').read() == open(fb, 'rb').read(), fa
-    ours_on_ref, ref_on_ours = tsv_io.TSVFile(b), rio.TSVFile(a)
-    assert len(ours_on_ref) == len(ref_on_ours) == 23
+    assert [file_digest(f) for f in _files(a)] == gold['files']
+    ours = tsv_io.TSVFile(a)
+    assert len(ours) == gold['len'] == 23
     for i in (0, 22, 9):
-        assert ours_on_ref[i] == ref_on_ours[i]
-        assert ours_on_ref.get_key(i) == ref_on_ours.get_key(i)
-    # merged parts: same .tsv and .lineidx.8b as the reference's concat (its process pool is bypassed: num_worker=0)
+        assert list(ours[i]) == gold['reads'][str(i)]['row']
+        assert ours.get_key(i) == gold['reads'][str(i)]['key']
+    # merged parts: same .tsv and .lineidx.8b as the reference's concat
     p1, p2 = str(tmp_path / 'p.0.2.tsv'), str(tmp_path / 'p.1.2.tsv')
     tsv_io.tsv_writer(iter(rows[:10]), p1)
     tsv_io.tsv_writer(iter(rows[10:]), p2)
-    o1, o2 = str(tmp_path / 'm_ours.tsv'), str(tmp_path / 'm_ref.tsv')
+    o1 = str(tmp_path / 'm_ours.tsv')
     tsv_io.concat_tsv_files([p1, p2], o1)
-    orig = rio.parallel_map
-    rio.parallel_map = lambda f, tasks, num_worker=0: [f(t) for t in tasks]
-    os.environ['GIT_TMP_FOLDER'] = str(tmp_path / 'tmp')
-    os.makedirs(os.path.join(os.environ['GIT_TMP_FOLDER'], str(tmp_path).lstrip('/')), exist_ok=True)
-    try:
-        rio.concat_tsv_files([p1, p2], o2)
-    finally:
-        rio.parallel_map = orig
-    assert open(o1, 'rb').read() == open(o2, 'rb').read()
-    assert open(_files(o1)[2], 'rb').read() == open(_files(o2)[2], 'rb').read()
+    assert file_digest(o1) == gold['concat']
+    assert file_digest(_files(o1)[2]) == gold['concat_lineidx_8b']

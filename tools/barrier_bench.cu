@@ -1,5 +1,5 @@
 // Grid-barrier micro-benchmark for the one-kernel decode step (tools/ only, not part of the library).
-// 148 CTAs x 256 threads, cooperative launch, N barriers back to back; between two barriers each CTA writes one word and
+// 132 CTAs (one per H100 SM) x 256 threads, cooperative launch, N barriers back to back; between two barriers each CTA writes one word and
 // reads its neighbour's (so a broken barrier shows as a wrong value).  Variants:
 //   0  flat counter: fence + red.release + ld.acquire spin   (what decode_mega_kernel does)
 //   1  flat counter without the __threadfence
@@ -68,15 +68,15 @@ __global__ void __launch_bounds__(256, 1) bench(unsigned* ctr, unsigned* flags, 
 template <int V>
 static void run(const char* name, int iters) {
   unsigned *ctr, *flags, *grp, *data; int* bad;
-  cudaMalloc(&ctr, 4096); cudaMalloc(&flags, 4096); cudaMalloc(&grp, 4096); cudaMalloc(&data, 148 * 128); cudaMalloc(&bad, 4);
+  cudaMalloc(&ctr, 4096); cudaMalloc(&flags, 4096); cudaMalloc(&grp, 4096); cudaMalloc(&data, 132 * 128); cudaMalloc(&bad, 4);
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   float best = 1e9f;
   int hbad = 0;
   for (int rep = 0; rep < 4; ++rep) {
-    cudaMemset(ctr, 0, 4096); cudaMemset(flags, 0, 4096); cudaMemset(grp, 0, 4096); cudaMemset(data, 0, 148 * 128); cudaMemset(bad, 0, 4);
+    cudaMemset(ctr, 0, 4096); cudaMemset(flags, 0, 4096); cudaMemset(grp, 0, 4096); cudaMemset(data, 0, 132 * 128); cudaMemset(bad, 0, 4);
     void* args[] = {&ctr, &flags, &grp, &data, &iters, &bad};
     cudaEventRecord(e0);
-    cudaError_t rc = cudaLaunchCooperativeKernel((void*)bench<V>, dim3(148), dim3(256), args, 0, 0);
+    cudaError_t rc = cudaLaunchCooperativeKernel((void*)bench<V>, dim3(132), dim3(256), args, 0, 0);
     cudaEventRecord(e1);
     if (rc != cudaSuccess || cudaEventSynchronize(e1) != cudaSuccess) { printf("%s: launch failed: %s\n", name, cudaGetErrorString(cudaGetLastError())); return; }
     float ms; cudaEventElapsedTime(&ms, e0, e1);
@@ -91,7 +91,7 @@ int main() {
   run<0>("0 flat counter, fence + red.release + ld.acquire spin", iters);
   run<1>("1 flat counter, no __threadfence", iters);
   run<4>("4 flat counter, ld.relaxed spin + fence", iters);
-  run<2>("2 flag all-gather (st.release flags[cta]; warp 0 polls 148 flags)", iters);
+  run<2>("2 flag all-gather (st.release flags[cta]; warp 0 polls 132 flags)", iters);
   run<3>("3 two-level counters (8 groups)", iters);
   return 0;
 }
