@@ -5,7 +5,7 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, 'libgitb200.so')
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 c_void_p, c_int, c_int64, c_float, c_char_p = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_char_p
 c_ll = ctypes.c_longlong
@@ -42,6 +42,7 @@ SIGNATURES = {
     'gitb200_finalize_weights': (c_int, [c_void_p, c_void_p]),
     'gitb200_share_weights': (c_int, [c_void_p, c_void_p]),
     'gitb200_set_input_size': (c_int, [c_void_p, c_int, c_int]),
+    'gitb200_set_image_sizes': (c_int, [c_void_p, ctypes.POINTER(ctypes.c_int32), c_int]),
     'gitb200_encode': (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
     'gitb200_prefill': (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
     'gitb200_decode_step': (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),

@@ -25,6 +25,7 @@ struct AttnParams {
   int B, S, H;
   long long q_rs, kv_rs, q_bs, kv_bs, o_rs, o_bs;  // row / batch strides in elements
   float scale_log2;                                 // (1/sqrt(64)) * log2(e)
+  const int* seq_lens;                              // flash_attn_wgmma_kernel<true>: [B] valid rows of each batch (<= S)
 };
 
 __device__ __forceinline__ void attn_load_tile(uint32_t smem_base, const __nv_bfloat16* g, long long row_stride,
@@ -196,6 +197,10 @@ __global__ void __launch_bounds__(NW * 32) flash_attn_kernel(const AttnParams p)
 constexpr int kAttnWgRows = 64;                 // query rows per CTA = keys per K / V block
 constexpr int kAttnWgSmem = 5 * 8192 + 64 + 1024;   // Q | K x 2 | V x 2 | barriers | alignment slack
 
+// kRagged (ragged image batches): batch b occupies a slot of p.S rows of which the first p.seq_lens[b] are valid; the
+// batch is computed exactly as a uniform call with S = seq_lens[b] would compute it (the key blocks and query tiles past
+// its length are skipped, not masked) and its output rows past that length are written as zeros.
+template <bool kRagged>
 __global__ void __launch_bounds__(128) flash_attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ,
                                                               const __grid_constant__ CUtensorMap tmK,
                                                               const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
@@ -206,10 +211,19 @@ __global__ void __launch_bounds__(128) flash_attn_wgmma_kernel(const __grid_cons
   uint8_t* sV = smem + 3 * 8192;
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 5 * 8192);   // [0] Q, [1 + stage] K | V
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int h = blockIdx.y, b = blockIdx.z, S = p.S;
+  const int h = blockIdx.y, b = blockIdx.z;
+  const int S = kRagged ? p.seq_lens[b] : p.S;
   const int q0 = blockIdx.x * kAttnWgRows;
-  const int row_base = b * S;                    // rows of batch b in the [B * S, H * 64] q / k / v views
+  const int row_base = b * p.S;                  // rows of batch b in the [B * S, H * 64] q / k / v views
   const int nblk = (S + kAttnWgRows - 1) / kAttnWgRows;
+  if (kRagged && q0 >= S) {                      // a query tile of the padding: zeros, no arithmetic
+    __nv_bfloat16* og = p.out + b * p.o_bs + h * 64;
+    for (int i = tid; i < kAttnWgRows * 8; i += 128) {
+      const int r = q0 + (i >> 3);
+      if (r < p.S) *reinterpret_cast<uint4*>(og + static_cast<long long>(r) * p.o_rs + (i & 7) * 8) = make_uint4(0, 0, 0, 0);
+    }
+    return;
+  }
   auto load_kv = [&](int blk, int st) {
     mbar_arrive_expect_tx(&bar[1 + st], 2 * 8192);
     tma_load_2d(sK + st * 8192, &tmK, &bar[1 + st], h * 64, row_base + blk * kAttnWgRows);
@@ -301,7 +315,9 @@ __global__ void __launch_bounds__(128) flash_attn_wgmma_kernel(const __grid_cons
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     if (r0 < S) *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r0) * p.o_rs + 8 * j) = pack_bf16(o[4 * j] * inv0, o[4 * j + 1] * inv0);
+    else if (kRagged && r0 < p.S) *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r0) * p.o_rs + 8 * j) = 0u;
     if (r1 < S) *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r1) * p.o_rs + 8 * j) = pack_bf16(o[4 * j + 2] * inv1, o[4 * j + 3] * inv1);
+    else if (kRagged && r1 < p.S) *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r1) * p.o_rs + 8 * j) = 0u;
   }
 }
 
@@ -330,7 +346,19 @@ struct DecAttnParams {
   int chunk_rows;                  // image keys staged per TMA round (<= 512), box_rows * n_boxes
   int box_rows;                    // rows per TMA box (<= 256)
   ChainSync chain;
+  const int* img_lens;             // decode_attn_kernel<., ., true>: [B] valid image keys of each image (M = slot length;
+                                   //   chunk_rows = the staging buffer's rows, box_rows = kDecAttnRaggedBox)
 };
+
+// Image keys of one (image, head) item are staged in chunks of at most kDecAttnChunk rows, all of one length: at least two
+// CTAs per SM fit (M = 257 in one piece would be 131 KB per CTA).  The chunking fixes which key group of the kernel sees
+// which key, so a ragged batch derives it from each image's own key count, as a uniform call of that image would.
+constexpr int kDecAttnChunk = 224;
+constexpr int kDecAttnRaggedBox = 32;   // ragged batches: rows per TMA box (the chunk length varies per image)
+__host__ __device__ __forceinline__ int dec_attn_chunk_rows(int M) {
+  const int n_chunks = (M + kDecAttnChunk - 1) / kDecAttnChunk;
+  return (M + n_chunks - 1) / n_chunks;
+}
 
 __device__ __forceinline__ void bf16x8_to_f32(const uint4& u, float (&f)[8]) {
   f[0] = bf16_lo(u.x); f[1] = bf16_hi(u.x);
@@ -380,7 +408,10 @@ __device__ __forceinline__ void dec_attn_update(float (&sc)[4], const uint4 (&w)
 // q/k/v of item k+1 are requested at the top of item k, and the text K/V rows of an item are requested before its
 // image-key loop (shared memory) and consumed after it.  At 256 rows a CTA walks ~10 items, so the exposed latencies
 // (not the HBM stream) bounded the kernel.
-template <int NQ, bool kPipe = false>
+//
+// kRagged: every image has its own key count img_lens[b] (<= M, the slot length) and chunk length, so each item is
+// computed exactly as in a uniform call of its image; the CTA's chunk sequence is no longer one fixed count per item.
+template <int NQ, bool kPipe = false, bool kRagged = false>
 __global__ void __launch_bounds__(128)
 decode_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, const DecAttnParams p) {
   constexpr bool kPipeOn = kPipe && NQ == 1;
@@ -400,7 +431,14 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
   const int G = gridDim.x;
   const int n_chunks = (p.M + p.chunk_rows - 1) / p.chunk_rows;
   const int n_my = (n_items - static_cast<int>(blockIdx.x) + G - 1) / G;
-  const int n_units = n_my * n_chunks;
+  int n_units = n_my * n_chunks;
+  if constexpr (kRagged) {
+    n_units = 0;
+    for (int k = 0; k < n_my; ++k) {
+      const int Mb = p.img_lens[(static_cast<int>(blockIdx.x) + k * G) / H];
+      n_units += (Mb + dec_attn_chunk_rows(Mb) - 1) / dec_attn_chunk_rows(Mb);
+    }
+  }
 
   griddep_launch_early();
   tl_mark(100003);
@@ -412,21 +450,27 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
     mbar_fence_init();
   }
   __syncthreads();
+  int iss_k = 0, iss_c = 0;       // kRagged: item / chunk of the next unit to fetch (thread 0 issues the units in order)
   auto issue_unit = [&](int u) {  // one thread
-    const int item = blockIdx.x + (u / n_chunks) * G;
-    const int c = u - (u / n_chunks) * n_chunks;
+    const int k = kRagged ? iss_k : u / n_chunks;
+    const int c = kRagged ? iss_c : u - k * n_chunks;
+    const int item = blockIdx.x + k * G;
     const int b = item / H, h = item - b * H;
     uint8_t* sK = sbase + static_cast<size_t>(u & 1) * 2 * kv_bytes;
     uint8_t* sV = sK + kv_bytes;
-    const int rows_c = min(p.chunk_rows, p.M - c * p.chunk_rows);
-    const int nb = (rows_c + p.box_rows - 1) / p.box_rows;
-    mbar_arrive_expect_tx(&bars[u & 1], static_cast<uint32_t>(2 * nb * p.box_rows * 128));
+    const int Mb = kRagged ? p.img_lens[b] : p.M;
+    const int crows = kRagged ? dec_attn_chunk_rows(Mb) : p.chunk_rows;
+    const int box = kRagged ? kDecAttnRaggedBox : p.box_rows;
+    const int rows_c = min(crows, Mb - c * crows);
+    const int nb = (rows_c + box - 1) / box;
+    mbar_arrive_expect_tx(&bars[u & 1], static_cast<uint32_t>(2 * nb * box * 128));
     for (int i = 0; i < nb; ++i) {
-      const int grow = b * p.M + c * p.chunk_rows + i * p.box_rows;
+      const int grow = b * p.M + c * crows + i * box;
       const int gcol = h * 64;
-      tma_load_2d(sK + static_cast<size_t>(i) * p.box_rows * 128, &tmK, &bars[u & 1], gcol, grow);
-      tma_load_2d(sV + static_cast<size_t>(i) * p.box_rows * 128, &tmV, &bars[u & 1], gcol, grow);
+      tma_load_2d(sK + static_cast<size_t>(i) * box * 128, &tmK, &bars[u & 1], gcol, grow);
+      tma_load_2d(sV + static_cast<size_t>(i) * box * 128, &tmV, &bars[u & 1], gcol, grow);
     }
+    if (kRagged && ++iss_c * crows >= Mb) { iss_c = 0; ++iss_k; }
   };
   if (tid == 0) {
     issue_unit(0);
@@ -492,9 +536,13 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
   };
   if (kPipeOn) request_qkv(kPre, nxt_a, nxt_b);   // items 0..kPre-1 were requested above
 
+  int u_base = 0;                 // units of the items before this one
   for (int k = 0; k < n_my; ++k) {
     const int item = blockIdx.x + k * G;
     const int b = item / H, h = item - b * H;
+    const int Mb = kRagged ? p.img_lens[b] : p.M;
+    const int crows = kRagged ? dec_attn_chunk_rows(Mb) : p.chunk_rows;
+    const int nch = kRagged ? (Mb + crows - 1) / crows : n_chunks;
     float cur_a = 0.f, cur_b = 0.f;
     if (kPipeOn && k >= kPre) {
       cur_a = nxt_a;
@@ -579,12 +627,12 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
       }
     }
     // ---- image keys from shared memory: shared by the NQ beams of this image ----
-    for (int c = 0; c < n_chunks; ++c) {
-      const int u_idx = k * n_chunks + c;
+    for (int c = 0; c < nch; ++c) {
+      const int u_idx = (kRagged ? u_base : k * n_chunks) + c;
       const uint8_t* sK = sbase + static_cast<size_t>(u_idx & 1) * 2 * kv_bytes;
       const uint8_t* sV = sK + kv_bytes;
       mbar_wait(&bars[u_idx & 1], static_cast<uint32_t>((u_idx >> 1) & 1));
-      const int rows_c = min(p.chunk_rows, p.M - c * p.chunk_rows);
+      const int rows_c = min(crows, Mb - c * crows);
       for (int base = 0; base < rows_c; base += 64) {  // uniform trip count: the shuffles below stay converged
         uint4 u[4], w[4];
 #pragma unroll
@@ -616,6 +664,7 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
       __syncthreads();  // everyone is done with this buffer: refill it with the unit after next
       if (tid == 0 && u_idx + 2 < n_units) issue_unit(u_idx + 2);
     }
+    u_base += nch;
     if (kPipeOn) {
       text_chunk_use(0, 0, tu, tw);
       for (int base = 64; base < n_txt; base += 64) {   // captions longer than 64 tokens: the rest the plain way
@@ -681,6 +730,7 @@ struct AttnF32Params {
   __nv_bfloat16* out;            // split3 rows: [S, 3 * d_model] per batch element
   int B, S, H, d_model;
   long long q_rs, kv_rs, q_bs, kv_bs, o_bs;   // row / batch strides in elements (output row stride = 3 * d_model)
+  const int* seq_lens;           // null, or [B] valid rows of each batch (ragged image batches): rows past it leave as zeros
 };
 
 __device__ __forceinline__ void store_split3_pair(__nv_bfloat16* row, int d_model, int col, float a, float b) {
@@ -702,6 +752,11 @@ __global__ void __launch_bounds__(128) attn_f32_kernel(const AttnF32Params p) {
   const int row = static_cast<int>(item % p.S);
   const int h = static_cast<int>((item / p.S) % p.H);
   const int b = static_cast<int>(item / (static_cast<long long>(p.S) * p.H));
+  const int S = p.seq_lens != nullptr ? p.seq_lens[b] : p.S;
+  if (row >= S) {
+    store_split3_pair(p.out + b * p.o_bs + static_cast<long long>(row) * 3 * p.d_model, p.d_model, h * 64 + 2 * lane, 0.f, 0.f);
+    return;
+  }
   const float* qg = p.q + b * p.q_bs + static_cast<long long>(row) * p.q_rs + h * 64;
   const float* kg = p.k + b * p.kv_bs + h * 64;
   const float* vg = p.v + b * p.kv_bs + h * 64;
@@ -709,9 +764,9 @@ __global__ void __launch_bounds__(128) attn_f32_kernel(const AttnF32Params p) {
   q_s[lane + 32] = qg[lane + 32] * 0.125f;
   __syncwarp();
   float mx = -INFINITY;
-  for (int j0 = 0; j0 < p.S; j0 += 32) {
+  for (int j0 = 0; j0 < S; j0 += 32) {
     const int j = j0 + lane;
-    if (j < p.S) {
+    if (j < S) {
       const float4* kr = reinterpret_cast<const float4*>(kg + static_cast<long long>(j) * p.kv_rs);
       float a = 0.f;
 #pragma unroll
@@ -726,7 +781,7 @@ __global__ void __launch_bounds__(128) attn_f32_kernel(const AttnF32Params p) {
   }
   mx = warp_max(mx);
   float sum = 0.f;
-  for (int j = lane; j < p.S; j += 32) {
+  for (int j = lane; j < S; j += 32) {
     const float e = expf(sc[j] - mx);
     sc[j] = e;
     sum += e;
@@ -734,7 +789,7 @@ __global__ void __launch_bounds__(128) attn_f32_kernel(const AttnF32Params p) {
   sum = warp_sum(sum);
   __syncwarp();
   float a0 = 0.f, a1 = 0.f;
-  for (int j = 0; j < p.S; ++j) {
+  for (int j = 0; j < S; ++j) {
     const float2 vv = *reinterpret_cast<const float2*>(vg + static_cast<long long>(j) * p.kv_rs + 2 * lane);
     a0 = fmaf(sc[j], vv.x, a0);
     a1 = fmaf(sc[j], vv.y, a1);
@@ -758,6 +813,7 @@ struct DecAttnF32Params {
   const StepState* state;
   int pos_fixed;
   ChainSync chain;
+  const int* img_lens;            // null, or [B] valid image keys of each image (ragged batches; M is the slot length)
 };
 
 // one warp per (sequence r, head h); 4 warps per CTA
@@ -776,7 +832,6 @@ __global__ void __launch_bounds__(128) decode_attn_f32_kernel(const DecAttnF32Pa
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int D = p.D, H = D / 64;
   const int pos = (p.state != nullptr) ? p.state->pos : p.pos_fixed;
-  const int n_keys = p.M + pos + 1;
   float* q_s = attn_f32_smem + warp * (192 + p.M + p.T_alloc);
   float* k_s = q_s + 64;
   float* v_s = q_s + 128;
@@ -785,6 +840,8 @@ __global__ void __launch_bounds__(128) decode_attn_f32_kernel(const DecAttnF32Pa
   if (item < p.R * H) {
     const int r = item / H, h = item - r * H;
     const int b = r / p.beam;
+    const int Mb = p.img_lens != nullptr ? p.img_lens[b] : p.M;
+    const int n_keys = Mb + pos + 1;
     const float* row = p.qkv + static_cast<long long>(r) * 3 * D + h * 64;
     const float* bias = p.bqkv + h * 64;
     for (int d = lane; d < 64; d += 32) {
@@ -798,8 +855,8 @@ __global__ void __launch_bounds__(128) decode_attn_f32_kernel(const DecAttnF32Pa
     }
     __syncwarp();
     auto key_ptr = [&](int j, bool want_v) -> const float* {   // row of key j (j != newest)
-      if (j < p.M) return (want_v ? p.img_v : p.img_k) + (static_cast<long long>(b) * p.M + j) * D + h * 64;
-      const int t = j - p.M;
+      if (j < Mb) return (want_v ? p.img_v : p.img_k) + (static_cast<long long>(b) * p.M + j) * D + h * 64;
+      const int t = j - Mb;
       const int pr = (p.src_row != nullptr) ? p.src_row[r * p.T_alloc + t] : r;
       return (want_v ? p.txt_v : p.txt_k) + (static_cast<long long>(pr) * p.T_alloc + t) * D + h * 64;
     };

@@ -9,6 +9,8 @@
 //                  hidden) bf16 row-major; packed qkv bf16 [NI*L, 3d].
 //   image K/V    : bf16 [layer][k|v][B][M][768]  (token-major rows: a decode-step reader streams contiguous
 //                  1536-byte rows; written once by the prefill QKV GEMM epilogue, shared by all beams).
+//                  Ragged batches (gitb200_set_image_sizes): M = L_max, image b's first L_b rows are valid and its
+//                  padding rows hold finite values that no valid row reads.
 //   text K/V     : bf16 [layer][k|v][rows][T_alloc][768] + int32 src_row[rows][T_alloc] indirection for beams.
 //   decode step  : fp32 row state [rows, 768], bf16 copy for the GEMMs, fp32 qkv / logits.
 #include <cuda.h>
@@ -39,7 +41,7 @@
 using namespace gitb200;
 typedef __nv_bfloat16 bf16;
 
-#define GITB200_ABI_VERSION 6
+#define GITB200_ABI_VERSION 7
 
 // ------------------------------------------------------------------------------------------------
 // errors
@@ -128,6 +130,12 @@ struct gitb200_engine {
   // input size of the next encode (gitb200_set_input_size; default image_size x image_size): patch grid gh x gw,
   // Lc = gh * gw + 1 tokens per image; differs from (g, g, L) for MinMaxResizeForTest inputs (reference inference.py:29-64)
   int in_h = 0, in_w = 0, gh = 0, gw = 0, Lc = 0;
+  // ragged batches: (height, width) of every image of the NEXT encode / generate (gitb200_set_image_sizes; consumed by it),
+  // and the per-image tables of the last encode (cur_ragged: its images had their own sizes; RaggedImg [B], L_b [B])
+  std::vector<int> rg_next_hw;
+  bool cur_ragged = false;
+  std::vector<int> cur_lens;
+  DevBuf rg_tab, rg_lens;
 
   // weights
   DevBuf w_patch, cls, pos_emb, lnpre_g, lnpre_b, lnpost_g, lnpost_b;
@@ -465,7 +473,9 @@ static int launch_attention_wgmma(gitb200_engine* h, const AttnParams& ap, cudaS
   TRY(get_tmap(h, ap.q, rows, ap.H * 64, ap.q_rs, kAttnWgRows, &tq));
   TRY(get_tmap(h, ap.k, rows, ap.H * 64, ap.kv_rs, kAttnWgRows, &tk));
   TRY(get_tmap(h, ap.v, rows, ap.H * 64, ap.kv_rs, kAttnWgRows, &tv));
-  flash_attn_wgmma_kernel<<<dim3((ap.S + kAttnWgRows - 1) / kAttnWgRows, ap.H, ap.B), 128, kAttnWgSmem, st>>>(tq, tk, tv, p);
+  const dim3 grid((ap.S + kAttnWgRows - 1) / kAttnWgRows, ap.H, ap.B);
+  if (ap.seq_lens != nullptr) flash_attn_wgmma_kernel<true><<<grid, 128, kAttnWgSmem, st>>>(tq, tk, tv, p);
+  else flash_attn_wgmma_kernel<false><<<grid, 128, kAttnWgSmem, st>>>(tq, tk, tv, p);
   CKL(h, "flash_attn_wgmma_kernel");
   return 0;
 }
@@ -473,6 +483,7 @@ static int launch_attention_wgmma(gitb200_engine* h, const AttnParams& ap, cudaS
 static int launch_attention(gitb200_engine* h, const AttnParams& ap, cudaStream_t st) {
   if (ap.q_bs == static_cast<long long>(ap.S) * ap.q_rs && ap.kv_bs == static_cast<long long>(ap.S) * ap.kv_rs)
     return launch_attention_wgmma(h, ap, st);
+  if (ap.seq_lens != nullptr) return fail(h, "attention: per-batch lengths need batches stored back to back");
   // flash_attn_kernel: batches with other strides
   AttnParams p = ap;
   p.scale_log2 = 0.125f * 1.44269504088896340736f;
@@ -602,6 +613,22 @@ extern "C" int gitb200_set_input_size(gitb200_engine* h, int height, int width) 
   return 0;
 }
 
+extern "C" int gitb200_set_image_sizes(gitb200_engine* h, const int32_t* hw_host, int n) {
+  if (!h) return 1;
+  if (h->pending) return fail(h, "set_image_sizes: a generate call is in flight");
+  if (!hw_host || n < 1) return fail(h, "set_image_sizes: bad argument");
+  const int p = h->cfg.patch;
+  std::vector<int> hw(hw_host, hw_host + 2 * n);
+  for (int b = 0; b < n; ++b) {
+    const int ih = hw[2 * b], iw = hw[2 * b + 1];
+    if (ih < p || iw < p) return fail(h, "set_image_sizes: image %d is %dx%d, smaller than one %dx%d patch", b, ih, iw, p, p);
+    const long long tokens = static_cast<long long>(ih / p) * (iw / p) + 1;
+    if (tokens > 16384) return fail(h, "set_image_sizes: image %d (%dx%d) gives %lld tokens (limit 16384)", b, ih, iw, tokens);
+  }
+  h->rg_next_hw.swap(hw);
+  return 0;
+}
+
 extern "C" int gitb200_create(const gitb200_config* cfg, int device, gitb200_engine** out) {
   gitb200_engine* h = nullptr;
   if (!cfg || !out) return fail(nullptr, "gitb200_create: null argument");
@@ -647,7 +674,7 @@ static void release_all(gitb200_engine* h) {
                     &h->pt, &h->pxd, &h->phd, &h->pq, &h->pctx, &h->pu, &h->img_kv, &h->txt_kv, &h->src_row[0],
                     &h->src_row[1], &h->xd_t, &h->hd_t, &h->qkv_t, &h->ctx_t, &h->t_t, &h->u_t, &h->logits, &h->state,
                     &h->next_token, &h->logprob_sum, &h->tokens_i64, &h->stage_img, &h->stage_tok, &h->stage_lp,
-                    &h->prefix_dev, &h->beam_ws, &h->sel_ws, &h->chain};
+                    &h->prefix_dev, &h->beam_ws, &h->sel_ws, &h->chain, &h->rg_tab, &h->rg_lens};
   for (DevBuf* b : bufs) b->release();
   for (auto& l : h->enc) {
     DevBuf* lb[] = {&l.wqkv, &l.bqkv, &l.wo, &l.bo, &l.ln1g, &l.ln1b, &l.ln2g, &l.ln2b, &l.w1, &l.b1, &l.w2, &l.b2};
@@ -891,24 +918,80 @@ extern "C" int gitb200_finalize_weights(gitb200_engine* h, void* stream) {
 // ------------------------------------------------------------------------------------------------
 // hot path A: encoder
 // ------------------------------------------------------------------------------------------------
+// Per-image tables of a ragged batch (hw: height, width of every image): RaggedImg [B] and L_b [B] on the device, the
+// positional embedding of every distinct patch grid of the call in h->pos_interp (the stored one copied for the model's
+// own grid, the bicubic re-sampling for any other), and the slot length L_max.
+static int ragged_setup(gitb200_engine* h, const std::vector<int>& hw, int B, int* L_max, cudaStream_t st) {
+  const int p = h->cfg.patch, d = h->d;
+  std::vector<RaggedImg> tab(B);
+  std::vector<std::pair<int, int>> grids;     // distinct (gh, gw) in order of first appearance
+  std::vector<int> grid_row;                  // their first row in the positional table
+  int rows = 0, Lm = 0;
+  long long off = 0;
+  for (int b = 0; b < B; ++b) {
+    RaggedImg& e = tab[b];
+    e.h = hw[2 * b]; e.w = hw[2 * b + 1];
+    e.gh = e.h / p; e.gw = e.w / p;
+    e.L = e.gh * e.gw + 1;
+    e.src_off = off;
+    off += 3LL * e.h * e.w;
+    size_t k = 0;
+    while (k < grids.size() && grids[k] != std::make_pair(e.gh, e.gw)) ++k;
+    if (k == grids.size()) { grids.emplace_back(e.gh, e.gw); grid_row.push_back(rows); rows += e.L; }
+    e.pos_row = grid_row[k];
+    Lm = std::max(Lm, e.L);
+  }
+  CK(h->pos_interp.ensure(static_cast<size_t>(rows) * d * 4));
+  for (size_t k = 0; k < grids.size(); ++k) {
+    const int gh = grids[k].first, gw = grids[k].second;
+    float* dst = h->pos_interp.as<float>() + static_cast<size_t>(grid_row[k]) * d;
+    if (gh == h->g && gw == h->g) {
+      CK(cudaMemcpyAsync(dst, h->pos_emb.p, static_cast<size_t>(h->L) * d * 4, cudaMemcpyDeviceToDevice, st));
+      continue;
+    }
+    const long long total = static_cast<long long>(gh * gw + 1) * (d / 4);
+    const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, h->num_sms * 8));
+    pos_embed_bicubic_kernel<<<grid, 256, 0, st>>>(h->pos_emb.as<float>(), dst, h->g, gh, gw, d);
+    CKL(h, "pos_embed_bicubic_kernel");
+  }
+  std::vector<int> lens(B);
+  for (int b = 0; b < B; ++b) lens[b] = tab[b].L;
+  CK(h->rg_tab.ensure(static_cast<size_t>(B) * sizeof(RaggedImg)));
+  CK(h->rg_lens.ensure(static_cast<size_t>(B) * 4));
+  CK(cudaMemcpyAsync(h->rg_tab.p, tab.data(), static_cast<size_t>(B) * sizeof(RaggedImg), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(h->rg_lens.p, lens.data(), static_cast<size_t>(B) * 4, cudaMemcpyHostToDevice, st));
+  h->cur_lens.swap(lens);
+  *L_max = Lm;
+  return 0;
+}
+
+// ragged_hw: empty, or (height, width) of each of the B images (gitb200_set_image_sizes; frames must be 1)
 static int encode_impl(gitb200_engine* h, const float* images, int B, int frames, bool list_input, float* feats_out,
-                       cudaStream_t st) {
+                       cudaStream_t st, const std::vector<int>& ragged_hw = std::vector<int>()) {
   if (!h->finalized) return fail(h, "weights not finalized");
   if (B < 1 || frames < 1) return fail(h, "encode: bad batch/frames");
+  const bool rg = !ragged_hw.empty();
+  if (rg && (static_cast<int>(ragged_hw.size()) != 2 * B || frames != 1))
+    return fail(h, "encode: %d image sizes were set for a batch of %d x %d frames (ragged batches take one frame)",
+                static_cast<int>(ragged_hw.size() / 2), B, frames);
   if (list_input && h->cfg.num_frames_emb > 0 && frames > h->cfg.num_frames_emb) {
     // reference zip() truncates to the number of temporal embeddings (layers/decoder.py:848-849)
     frames = h->cfg.num_frames_emb;
   }
-  const int d = h->d, L = h->Lc, gh = h->gh, gw = h->gw, Kp = h->Kp, H = h->cfg.enc_heads;
+  h->cur_ragged = false;
+  int L = h->Lc;
+  if (rg) TRY(ragged_setup(h, ragged_hw, B, &L, st));
+  const int d = h->d, gh = h->gh, gw = h->gw, Kp = h->Kp, H = h->cfg.enc_heads;
   const int NI = B * frames;
   const long long Me = static_cast<long long>(NI) * L;
   const int ks = h->ks();                 // parity mode: GEMM operands are [hi | lo | hi] -> 3x the K extent
   const bool par = h->parity;
+  const int* seq_lens = rg ? h->rg_lens.as<int>() : nullptr;
   CK(h->x.ensure(Me * d * 4));
   CK(h->h.ensure(Me * d * 2 * ks));
   CK(h->qkv.ensure(Me * 3 * d * (par ? 4 : 2)));         // parity: q | k | v stay fp32
   CK(h->ctx.ensure(Me * d * 2 * ks));
-  CK(h->u.ensure(std::max<long long>(Me * 4 * d * 2, static_cast<long long>(NI) * gh * gw * Kp * 2) * ks));
+  CK(h->u.ensure(std::max<long long>(Me * 4 * d * 2, static_cast<long long>(NI) * (L - 1) * Kp * 2) * ks));
   CK(h->feats.ensure(Me * d * 2 * ks));
   float* x = h->x.as<float>();
   bf16* hb = h->h.as<bf16>();
@@ -918,8 +1001,9 @@ static int encode_impl(gitb200_engine* h, const float* images, int B, int frames
 
   // positional embedding of this input size: the stored one, or its bicubic re-sampling to the gh x gw grid
   // (reference layers/CLIP/model.py:245-251; recomputed per call: 1 + gh*gw rows, the parameters may have changed)
-  const float* pos = h->pos_emb.as<float>();
-  if (gh != h->g || gw != h->g) {
+  // (ragged batches: one table per distinct grid, made by ragged_setup)
+  const float* pos = rg ? h->pos_interp.as<float>() : h->pos_emb.as<float>();
+  if (!rg && (gh != h->g || gw != h->g)) {
     CK(h->pos_interp.ensure(static_cast<size_t>(L) * d * 4));
     const long long total = static_cast<long long>(L) * (d / 4);
     const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, h->num_sms * 8));
@@ -928,19 +1012,26 @@ static int encode_impl(gitb200_engine* h, const float* images, int B, int frames
     pos = h->pos_interp.as<float>();
   }
   // patch embedding: im2col + GEMM, rows land at token index 1 + patch (CLS row is filled by the next kernel)
+  // (ragged batches: every image owns L_max - 1 patch rows, the ones past its own grid are zero)
   {
-    const long long total = static_cast<long long>(NI) * gh * gw * (Kp / 8);
+    const long long total = static_cast<long long>(NI) * (L - 1) * (Kp / 8);
     const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, h->num_sms * 16));
-    im2col_patch_kernel<<<grid, 256, 0, st>>>(images, u, NI, h->in_h, h->in_w, h->cfg.patch, gh, gw, Kp, par ? 1 : 0);
+    if (rg) im2col_patch_ragged_kernel<<<grid, 256, 0, st>>>(images, u, h->rg_tab.as<RaggedImg>(), NI, L - 1, h->cfg.patch, Kp, par ? 1 : 0);
+    else im2col_patch_kernel<<<grid, 256, 0, st>>>(images, u, NI, h->in_h, h->in_w, h->cfg.patch, gh, gw, Kp, par ? 1 : 0);
     CKL(h, "im2col_patch_kernel");
-    GemmCall c = gemm_plain(u, Kp * ks, h->w_patch.as<bf16>(), Kp * ks, NI * gh * gw, d, Kp * ks, nullptr, ACT_NONE, nullptr, x, false);
-    c.p.rows_per_batch = gh * gw;
+    GemmCall c = gemm_plain(u, Kp * ks, h->w_patch.as<bf16>(), Kp * ks, NI * (L - 1), d, Kp * ks, nullptr, ACT_NONE, nullptr, x, false);
+    c.p.rows_per_batch = L - 1;
     c.p.batch_stride = L;
     c.p.row_offset = 1;
     TRY(launch_gemm(h, c, st));
     const int gridr = static_cast<int>((Me + 7) / 8);
-    if (d == 768)
+    const RaggedImg* tab = h->rg_tab.as<RaggedImg>();
+    if (d == 768 && rg)
+      cls_pos_lnpre_kernel<768, true><<<gridr, 256, 0, st>>>(x, h->cls.as<float>(), pos, h->lnpre_g.as<float>(), h->lnpre_b.as<float>(), static_cast<int>(Me), L, tab);
+    else if (d == 768)
       cls_pos_lnpre_kernel<768><<<gridr, 256, 0, st>>>(x, h->cls.as<float>(), pos, h->lnpre_g.as<float>(), h->lnpre_b.as<float>(), static_cast<int>(Me), L);
+    else if (rg)
+      cls_pos_lnpre_kernel<1024, true><<<gridr, 256, 0, st>>>(x, h->cls.as<float>(), pos, h->lnpre_g.as<float>(), h->lnpre_b.as<float>(), static_cast<int>(Me), L, tab);
     else
       cls_pos_lnpre_kernel<1024><<<gridr, 256, 0, st>>>(x, h->cls.as<float>(), pos, h->lnpre_g.as<float>(), h->lnpre_b.as<float>(), static_cast<int>(Me), L);
     CKL(h, "cls_pos_lnpre_kernel");
@@ -961,6 +1052,7 @@ static int encode_impl(gitb200_engine* h, const float* images, int B, int frames
       ap.B = NI; ap.S = L; ap.H = H; ap.d_model = d;
       ap.q_rs = 3 * d; ap.kv_rs = 3 * d; ap.q_bs = static_cast<long long>(L) * 3 * d; ap.kv_bs = ap.q_bs;
       ap.o_bs = static_cast<long long>(L) * 3 * d;
+      ap.seq_lens = seq_lens;
       TRY(launch_attention_f32(h, ap, st));
     } else {
       AttnParams ap{};
@@ -968,6 +1060,7 @@ static int encode_impl(gitb200_engine* h, const float* images, int B, int frames
       ap.B = NI; ap.S = L; ap.H = H;
       ap.q_rs = 3 * d; ap.kv_rs = 3 * d; ap.q_bs = static_cast<long long>(L) * 3 * d; ap.kv_bs = ap.q_bs;
       ap.o_rs = d; ap.o_bs = static_cast<long long>(L) * d;
+      ap.seq_lens = seq_lens;
       TRY(launch_attention(h, ap, st));
     }
     TRY(launch_gemm(h, gemm_plain(ctx, d * ks, l.wo.as<bf16>(), d * ks, static_cast<int>(Me), d, d * ks, l.bo.as<float>(), ACT_NONE, x, x, false), st));
@@ -992,6 +1085,7 @@ static int encode_impl(gitb200_engine* h, const float* images, int B, int frames
   h->cur_B = B;
   h->cur_frames = frames;
   h->cur_M = frames * L;
+  h->cur_ragged = rg;
   return 0;
 }
 
@@ -1085,12 +1179,14 @@ static int prefill_impl(gitb200_engine* h, int B, int beam, int T_alloc, float* 
       ap.v = reinterpret_cast<const float*>(img_kv_ptr(h, j, 1)); ap.out = ctx;
       ap.B = B; ap.S = M; ap.H = H; ap.d_model = D;
       ap.q_rs = D; ap.kv_rs = D; ap.q_bs = static_cast<long long>(M) * D; ap.kv_bs = ap.q_bs; ap.o_bs = 3 * ap.q_bs;
+      ap.seq_lens = h->cur_ragged ? h->rg_lens.as<int>() : nullptr;
       TRY(launch_attention_f32(h, ap, st));
     } else {
       AttnParams ap{};
       ap.q = q; ap.k = reinterpret_cast<const bf16*>(img_kv_ptr(h, j, 0)); ap.v = reinterpret_cast<const bf16*>(img_kv_ptr(h, j, 1)); ap.out = ctx;
       ap.B = B; ap.S = M; ap.H = H;
       ap.q_rs = D; ap.kv_rs = D; ap.q_bs = static_cast<long long>(M) * D; ap.kv_bs = ap.q_bs; ap.o_rs = D; ap.o_bs = ap.q_bs;
+      ap.seq_lens = h->cur_ragged ? h->rg_lens.as<int>() : nullptr;
       TRY(launch_attention(h, ap, st));
     }
     TRY(launch_gemm(h, gemm_plain(ctx, D * ks, l.wo.as<bf16>(), D * ks, static_cast<int>(rows), D, D * ks, l.bo.as<float>(), ACT_NONE, xd, t, false), st));
@@ -1174,6 +1270,7 @@ static int step_layers(gitb200_engine* h, Lane& ln_, const long long* tokens, co
       ap.src_row = src_row; ap.ctx = ctx; ap.R = R; ap.beam = beam; ap.M = h->cur_M; ap.T_alloc = h->T_alloc; ap.D = D;
       ap.state = state;
       ap.chain = cs;
+      ap.img_lens = h->cur_ragged ? h->rg_lens.as<int>() : nullptr;
       const size_t smem = static_cast<size_t>(4) * (192 + h->cur_M + h->T_alloc) * sizeof(float);
       if (smem > 200 * 1024) return fail(h, "parity decode attention: %d keys do not fit in shared memory", h->cur_M + h->T_alloc);
       CK(cudaFuncSetAttribute(decode_attn_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
@@ -1191,11 +1288,18 @@ static int step_layers(gitb200_engine* h, Lane& ln_, const long long* tokens, co
       ap.state = state;
       ap.chunk_rows = h->attn_chunk_rows; ap.box_rows = h->attn_box_rows;
       ap.chain = cs;
+      ap.img_lens = h->cur_ragged ? h->rg_lens.as<int>() : nullptr;
       CUtensorMap tk, tv;
       TRY(get_tmap(h, ap.img_k, static_cast<long long>(ln_.nb) * h->cur_M, D, D, ap.box_rows, &tk, false));
       TRY(get_tmap(h, ap.img_v, static_cast<long long>(ln_.nb) * h->cur_M, D, D, ap.box_rows, &tv, false));
       dim3 grid(std::min(h->attn_grid, ln_.nb * h->cfg.dec_heads));
-      if (beam == 1) CK(launch_k(pdl, decode_attn_kernel<1, true>, grid, dim3(128), h->attn_smem, st, tk, tv, ap));
+      if (h->cur_ragged) {
+        if (beam == 1) CK(launch_k(pdl, decode_attn_kernel<1, true, true>, grid, dim3(128), h->attn_smem, st, tk, tv, ap));
+        else if (beam == 4) CK(launch_k(pdl, decode_attn_kernel<4, false, true>, grid, dim3(128), h->attn_smem, st, tk, tv, ap));
+        else if (beam == 3) CK(launch_k(pdl, decode_attn_kernel<3, false, true>, grid, dim3(128), h->attn_smem, st, tk, tv, ap));
+        else if (beam == 2) CK(launch_k(pdl, decode_attn_kernel<2, false, true>, grid, dim3(128), h->attn_smem, st, tk, tv, ap));
+        else return fail(h, "decode: beam size %d not supported (1 .. 4)", beam);
+      } else if (beam == 1) CK(launch_k(pdl, decode_attn_kernel<1, true>, grid, dim3(128), h->attn_smem, st, tk, tv, ap));
       else if (beam == 4) CK(launch_k(pdl, decode_attn_kernel<4>, grid, dim3(128), h->attn_smem, st, tk, tv, ap));
       else if (beam == 3) CK(launch_k(pdl, decode_attn_kernel<3>, grid, dim3(128), h->attn_smem, st, tk, tv, ap));
       else if (beam == 2) CK(launch_k(pdl, decode_attn_kernel<2>, grid, dim3(128), h->attn_smem, st, tk, tv, ap));
@@ -1229,6 +1333,14 @@ static int set_attn_smem_limit(gitb200_engine* h) {
   const int n_chunks = (M + 223) / 224;
   h->attn_box_rows = (M + n_chunks - 1) / n_chunks;
   h->attn_chunk_rows = h->attn_box_rows;
+  if (h->cur_ragged) {
+    // every image is chunked by its own key count (dec_attn_chunk_rows) and fetched in 32-row boxes: the staging buffer
+    // holds the longest chunk of the call rounded up to whole boxes
+    int rows = 0;
+    for (int Lb : h->cur_lens) rows = std::max(rows, dec_attn_chunk_rows(Lb));
+    h->attn_box_rows = kDecAttnRaggedBox;
+    h->attn_chunk_rows = (rows + kDecAttnRaggedBox - 1) / kDecAttnRaggedBox * kDecAttnRaggedBox;
+  }
   h->attn_smem = static_cast<size_t>(4) * h->attn_chunk_rows * 128 + 128;
   int per_sm = static_cast<int>((227 * 1024) / (h->attn_smem + 8 * 1024));
   per_sm = std::max(1, std::min(per_sm, 4));
@@ -1238,6 +1350,12 @@ static int set_attn_smem_limit(gitb200_engine* h) {
   CK(cudaFuncSetAttribute(decode_attn_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(h->attn_smem)));
   CK(cudaFuncSetAttribute(decode_attn_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(h->attn_smem)));
   CK(cudaFuncSetAttribute(decode_attn_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(h->attn_smem)));
+  if (h->cur_ragged) {
+    CK(cudaFuncSetAttribute(decode_attn_kernel<1, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(h->attn_smem)));
+    CK(cudaFuncSetAttribute(decode_attn_kernel<4, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(h->attn_smem)));
+    CK(cudaFuncSetAttribute(decode_attn_kernel<3, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(h->attn_smem)));
+    CK(cudaFuncSetAttribute(decode_attn_kernel<2, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(h->attn_smem)));
+  }
   CK(h->chain.ensure(256));
   CK(cudaMemset(h->chain.p, 0, 256));
   return 0;

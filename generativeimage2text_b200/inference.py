@@ -352,9 +352,10 @@ def test_git_inference_single_tsv(image_tsv, model_name, question_tsv, out_tsv, 
         return key, img
 
     def caption_rows():
-        """Batches of decoded rows -> GPU transform -> model.submit with `depth` batches in flight."""
+        """Batches of decoded rows -> GPU transform -> model.submit with `depth` batches in flight.  With
+        `test_respect_ratio_max` every image has its own size: batches of more than one image go out as ragged lists."""
         variable = transforms.minmax is not None
-        bs = 1 if variable else max(1, batch_size)
+        bs = max(1, batch_size)
         pending = []
 
         def drain(item):
@@ -367,14 +368,47 @@ def test_git_inference_single_tsv(image_tsv, model_name, question_tsv, out_tsv, 
             rows = list(pool.map(decode_row, idx[b0:b0 + bs]))
             keys = [k for k, _ in rows]
             t = transforms.batch([im for _, im in rows])
-            x = t if not variable else t[0]
+            x = t if not variable else (t[0] if bs == 1 else [im[0] for im in t])
             pending.append((keys, model.submit({'image': x}, depth=depth)))
             if len(pending) >= depth:
                 yield from drain(pending.pop(0))
         while pending:
             yield from drain(pending.pop(0))
 
+    def question_rows_ragged(group):
+        """Up to `group` consecutive images with all their questions in ONE ragged call: the image repeated once per
+        question, one prefix per row (as the per-image question batch below)."""
+        idx = list(range(curr_start, curr_end))
+        for b0 in range(0, len(idx), group):
+            images, questions, ids = [], [], []
+            for i in idx[b0:b0 + group]:
+                image_key, image_col = image_tsv[i][:2]
+                q_key, q_info = question_tsv[i][:2]
+                assert image_key == q_key
+                img = transforms(pilimg_from_base64(image_col))
+                for q in json.loads(q_info):
+                    images.append(img)
+                    questions.append(q)
+                    ids.append(_prefix_ids(tokenizer, q['question']))
+            if not ids:
+                continue
+            with torch.no_grad():
+                if len(ids) == 1:
+                    result = model({'image': images, 'prefix': torch.tensor(ids[0]).unsqueeze(0).cuda()})
+                else:
+                    width = max(len(i) for i in ids)
+                    pad = torch.zeros((len(ids), width), dtype=torch.long)
+                    for r, i in enumerate(ids):
+                        pad[r, :len(i)] = torch.tensor(i)
+                    result = model({'image': images, 'prefix': pad.cuda(), 'prefix_len': torch.tensor([len(i) for i in ids])})
+            for q, p in zip(questions, result['predictions'].tolist()):
+                answer = tokenizer.decode(p, skip_special_tokens=True)
+                yield json_dump({'answer': answer, 'question_id': q['question_id']}),
+
     def question_rows():
+        if transforms.minmax is not None and batch_size > 1:
+            yield from question_rows_ragged(batch_size)
+            return
         for i in range(curr_start, curr_end):
             image_key, image_col = image_tsv[i][:2]
             q_key, q_info = question_tsv[i][:2]

@@ -418,6 +418,40 @@ class GitB200CaptioningModel(nn.Module):
         raise TypeError('model.decoder must be an AutoRegressiveBeamSearch, TrieAutoRegressiveBeamSearch or GeneratorWithBeamSearch '
                         'of this package')
 
+    @staticmethod
+    def _is_ragged(image):
+        """A list of 3-D [3, H_b, W_b] tensors = B single images of their own sizes (a list of 4-D tensors = video frames)."""
+        if not isinstance(image, (list, tuple)) or not image:
+            return False
+        dims = [im.dim() for im in image]
+        if 3 in dims and any(n != 3 for n in dims):
+            raise ValueError('a ragged batch is a list of [3, H, W] images; it cannot be mixed with [B, 3, H, W] frames')
+        return dims[0] == 3
+
+    def _pack_ragged(self, image):
+        """List of [3, H_b, W_b] images -> (the B images back to back as one fp32 vector on the device, B, [(H_b, W_b)])."""
+        enc = ENCODER_CFG[self.param.get('image_encoder_type', 'CLIPViT_B_16')]
+        sizes = []
+        for b, im in enumerate(image):
+            if im.shape[0] != 3:
+                raise ValueError('image %d of a ragged batch must be [3, H, W] (got %s)' % (b, tuple(im.shape)))
+            if im.shape[1] < enc['patch'] or im.shape[2] < enc['patch']:
+                raise ValueError('image %d (%s) is smaller than one patch' % (b, tuple(im.shape[1:])))
+            sizes.append((int(im.shape[1]), int(im.shape[2])))
+        dev = self._device()
+        x = torch.cat([im.to(device=dev, dtype=torch.float32, non_blocking=True).reshape(-1) for im in image])
+        return x, len(sizes), sizes
+
+    def _image_tokens(self, sizes):
+        """Image tokens L_b of each (H_b, W_b): the patch grid plus the class token."""
+        p = ENCODER_CFG[self.param.get('image_encoder_type', 'CLIPViT_B_16')]['patch']
+        return [(h // p) * (w // p) + 1 for h, w in sizes]
+
+    @staticmethod
+    def _sizes_arg(sizes):
+        """(int32 [n][2] host array of the sizes, n) for gitb200_set_image_sizes."""
+        return (ctypes.c_int32 * (2 * len(sizes)))(*[v for hw in sizes for v in hw]), len(sizes)
+
     def _pack_images(self, image):
         """-> (fp32 contiguous [frames*B,3,S,S] on device, B, frames) ; frames = 0 for a bare tensor."""
         dev = self._device()
@@ -445,7 +479,9 @@ class GitB200CaptioningModel(nn.Module):
         """`model(batch)` of the reference in eval mode: CaptioningModel.forward -> infer.
 
         batch: {'image': FloatTensor[B,3,H,W] | [FloatTensor[B,3,H,W]] * frames, 'prefix'?: LongTensor[1,P]}
-               (extension: 'prefix': LongTensor[B,P] + optional 'prefix_len': [B] = one prefix per image)
+               (extension: 'prefix': LongTensor[B,P] + optional 'prefix_len': [B] = one prefix per image;
+               extension: 'image': [FloatTensor[3,H_b,W_b]] * B = B single images of their own sizes (ragged batch): row b is
+               what `model({'image': image[b][None]})` returns, no temporal embedding)
         forced_tokens / return_step_logits are parity-test hooks (teacher forcing, raw per-step logits).
         search_param: the dict CaptioningModel.infer forwards to decoder.search (layers/decoder.py:999-1003); understood:
                {'do_sample': True, 'temperature': T, 'top_k': ., 'top_p': .} with the greedy decoder -- top_k / top_p are
@@ -472,7 +508,8 @@ class GitB200CaptioningModel(nn.Module):
             raise NotImplementedError("'context' batches are not produced by the reference inference path")
         search_param = dict(search_param or {})
         constrained = bool(search_param) or isinstance(self.decoder, TrieAutoRegressiveBeamSearch)
-        if (int(coalesce) > 1 and slot is None and not _caller_stream and forced_tokens is None and not return_step_logits
+        ragged = self._is_ragged(batch['image'])     # a ragged batch is launched on its own (never coalesced)
+        if (int(coalesce) > 1 and not ragged and slot is None and not _caller_stream and forced_tokens is None and not return_step_logits
                 and 'prefix' not in batch and 'prefix_len' not in batch and not constrained):
             return self._submit_coalesced(batch['image'], depth, int(coalesce))
         if self._open_group is not None:
@@ -488,7 +525,12 @@ class GitB200CaptioningModel(nn.Module):
         eng = sl['engine']
         dev = self._device()
         cur = torch.cuda.current_stream(dev)
-        x, B, frames = self._pack_images(batch['image'])      # (copies / casts, if any, run on the caller's stream)
+        # (copies / casts, if any, run on the caller's stream)
+        if ragged:
+            x, B, sizes = self._pack_ragged(batch['image'])
+            frames = 0
+        else:
+            x, B, frames = self._pack_images(batch['image'])
         if _caller_stream:
             stream = cur                      # synchronous path: the caller's stream (stream 0 -> engine-owned stream)
         else:
@@ -538,7 +580,11 @@ class GitB200CaptioningModel(nn.Module):
                 t.record_stream(stream)
         # inputs of another size than test_crop_size (MinMaxResizeForTest, reference inference.py:29-64): the engine
         # re-samples the positional embedding to their patch grid (reference layers/CLIP/model.py:245-251)
-        _lib.check(lib.gitb200_set_input_size(eng, int(x.shape[-2]), int(x.shape[-1])), eng, 'set_input_size')
+        # (a ragged batch: every image's own size, for this call only)
+        if ragged:
+            _lib.check(lib.gitb200_set_image_sizes(eng, *self._sizes_arg(sizes)), eng, 'set_image_sizes')
+        else:
+            _lib.check(lib.gitb200_set_input_size(eng, int(x.shape[-2]), int(x.shape[-1])), eng, 'set_input_size')
         if row_prefix is not None:
             _lib.check(lib.gitb200_set_row_prefixes(eng, row_prefix.data_ptr(), B, int(row_prefix.shape[1]), row_lens_dev.data_ptr()),
                        eng, 'set_row_prefixes')
@@ -671,10 +717,19 @@ class GitB200CaptioningModel(nn.Module):
     # ---------------------------------------------------------------- parity hooks (intermediate activations)
     @torch.no_grad()
     def encode_image(self, image):
-        """Image features as the decoder sees them: [B, frames*L, d] fp32 (reference layers/decoder.py:846-857)."""
+        """Image features as the decoder sees them: [B, frames*L, d] fp32 (reference layers/decoder.py:846-857); for a ragged
+        list of [3, H_b, W_b] images, a list of [1, L_b, d] (image b alone, as `encode_image(image[b][None])` gives it)."""
         lib, stream = self._ensure_engine()
-        x, B, frames = self._pack_images(image)
         enc = ENCODER_CFG[self.param.get('image_encoder_type', 'CLIPViT_B_16')]
+        if self._is_ragged(image):
+            x, B, sizes = self._pack_ragged(image)
+            lens = self._image_tokens(sizes)
+            feats = torch.empty((B, max(lens), enc['width']), dtype=torch.float32, device=x.device)
+            self._m_tokens = max(lens)
+            _lib.check(lib.gitb200_set_image_sizes(self._engine, *self._sizes_arg(sizes)), self._engine, 'set_image_sizes')
+            _lib.check(lib.gitb200_encode(self._engine, x.data_ptr(), B, 0, feats.data_ptr(), stream), self._engine, 'encode')
+            return [feats[b:b + 1, :n] for b, n in enumerate(lens)]
+        x, B, frames = self._pack_images(image)
         L = (x.shape[-2] // enc['patch']) * (x.shape[-1] // enc['patch']) + 1
         _lib.check(lib.gitb200_set_input_size(self._engine, int(x.shape[-2]), int(x.shape[-1])), self._engine, 'set_input_size')
         nf = max(frames, 1)

@@ -13,6 +13,7 @@ import mmap
 import os
 import os.path as op
 import shutil
+import threading
 
 import numpy as np
 
@@ -91,6 +92,9 @@ def concat_tsv_files(tsvs, out_tsv):
     merged.astype('<i8').tofile(_lineidx_names(out_tsv)[1])
 
 
+_OPEN_LOCK = threading.Lock()
+
+
 class TSVFile(object):
     """Random access to the rows of a TSV through its `.lineidx.8b` (reference tsv_io.py:121-352).
 
@@ -152,12 +156,18 @@ class TSVFile(object):
 
     # -- data ----------------------------------------------------------------------------------------------------
     def _ensure_tsv_opened(self):
-        if self._mfp is not None and self.pid != os.getpid():     # forked worker: re-open (reference tsv_io.py:345-350)
-            self.close_fp()
-        if self._mfp is None:
-            self._fp = open(self.tsv_file, 'rb')
-            self._mfp = mmap.mmap(self._fp.fileno(), 0, access=mmap.ACCESS_READ) if self.tsv_file_size else b''
-            self.pid = os.getpid()
+        if self._mfp is not None and self.pid == os.getpid():
+            return
+        # threads of one process (the TSV driver decodes rows on a thread pool) open the file once: without the lock a
+        # second opener replaced self._fp and closed the file another thread was about to map
+        with _OPEN_LOCK:
+            if self._mfp is not None and self.pid != os.getpid():     # forked worker: re-open (reference tsv_io.py:345-350)
+                self.close_fp()
+            if self._mfp is None:
+                fp = open(self.tsv_file, 'rb')
+                self._mfp = mmap.mmap(fp.fileno(), 0, access=mmap.ACCESS_READ) if self.tsv_file_size else b''
+                self._fp = fp
+                self.pid = os.getpid()
 
     def row_bytes(self, i):
         self._ensure_tsv_opened()

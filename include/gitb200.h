@@ -84,8 +84,9 @@ int gitb200_share_weights(gitb200_engine* h, gitb200_engine* src);
 /* Replaces: CaptioningModel.forward_one image branch = VisualTransformer.forward per frame
  * (+ img_temperal_embedding, token-axis concat)      layers/decoder.py:846-857, layers/CLIP/model.py:240-268.
  * images_dev: fp32 [frames][B,3,H,W] contiguous (frames >= 1; frame f at offset f*B*3*H*W; H = W = image_size unless
- * gitb200_set_input_size says otherwise).
- * feats_out_dev: fp32 [B, frames*L, enc_width] or NULL (kept internally for gitb200_prefill). */
+ * gitb200_set_input_size says otherwise), or B images of their own sizes back to back (gitb200_set_image_sizes).
+ * feats_out_dev: fp32 [B, frames*L, enc_width] or NULL (kept internally for gitb200_prefill); [B, L_max, enc_width] for
+ * images of their own sizes (image b's first L_b rows are its features, the rest finite padding). */
 int gitb200_encode(gitb200_engine* h, const float* images_dev, int batch, int frames, float* feats_out_dev,
                    void* stream);
 
@@ -93,8 +94,18 @@ int gitb200_encode(gitb200_engine* h, const float* images_dev, int batch, int fr
  * (MinMaxResizeForTest inputs, inference.py:29-64): the patch grid becomes (height / patch) x (width / patch) and the
  * positional embedding is re-sampled to it on the device, bicubic, as VisualTransformer.forward does at run time
  *                                                                                  layers/CLIP/model.py:245-251.
- * All images of one call share the size.  Sticky until changed; gitb200_create starts at image_size x image_size. */
+ * All images of one call share the size (gitb200_set_image_sizes gives every image its own).  Sticky until changed;
+ * gitb200_create starts at image_size x image_size. */
 int gitb200_set_input_size(gitb200_engine* h, int height, int width);
+
+/* Ragged batches: every image of the NEXT gitb200_encode / gitb200_generate* call has its own size (MinMaxResizeForTest
+ * inputs of different aspect ratios in one call).  hw_host: int32 [n][2] = (height, width) of each image; that call's
+ * images (images_dev or the host buffer) hold the n images back to back, fp32 [3, H_b, W_b] each; its batch must equal n
+ * and frames must be 0 or 1.  Image b has L_b = (H_b / patch) * (W_b / patch) + 1 tokens in a slot of L_max = max L_b
+ * rows: row b of the results is what a batch-1 call with that image alone returns.  The greedy decode steps of such a
+ * call run on the kernel chain (use_mega does not apply).  Applies to the next call only, like gitb200_set_row_prefixes;
+ * gitb200_set_input_size is left as it was. */
+int gitb200_set_image_sizes(gitb200_engine* h, const int32_t* hw_host, int n);
 
 /* Replaces: visual_projection + the image rows of BertEncoderAsDecoder, computed once (KV cache)
  *                                      layers/decoder.py:535, 92-174; layers/bert/modeling_bert.py:92-334.
