@@ -41,7 +41,7 @@
 using namespace gitb200;
 typedef __nv_bfloat16 bf16;
 
-#define GITB200_ABI_VERSION 7
+#define GITB200_ABI_VERSION 8
 
 // ------------------------------------------------------------------------------------------------
 // errors
@@ -517,6 +517,76 @@ static int launch_attention_f32(gitb200_engine* h, const AttnF32Params& p, cudaS
   const long long items = static_cast<long long>(p.B) * p.H * p.S;
   attn_f32_kernel<<<static_cast<unsigned int>((items + 3) / 4), 128, smem, st>>>(p);
   CKL(h, "attn_f32_kernel");
+  return 0;
+}
+
+// Geometry of decode_attn_kernel for image slots of M keys (lens: null, or the n valid key counts of a ragged batch) and
+// `items` (image, head) pairs.  The image K/V slice of one item is M rows of 128 B, staged in chunks of at most
+// kDecAttnChunk rows: two (K + V) staging buffers of one chunk per CTA, and at least two CTAs per SM (M = 257 in one piece
+// would be 131 KB per CTA = one 4-warp CTA per SM).  A uniform chunk is one TMA box.
+struct DecAttnGeom {
+  int chunk_rows, box_rows;   // DecAttnParams::chunk_rows / box_rows
+  size_t smem;                // dynamic shared memory per CTA
+  int grid;                   // CTAs the engine launches
+};
+static DecAttnGeom dec_attn_geometry(int M, const int* lens, int n, int num_sms, int items) {
+  DecAttnGeom g;
+  g.box_rows = g.chunk_rows = dec_attn_chunk_rows(M);
+  if (lens != nullptr) {
+    // every image is chunked by its own key count (dec_attn_chunk_rows) and fetched in 32-row boxes: the staging buffer
+    // holds the longest chunk of the call rounded up to whole boxes
+    int rows = 0;
+    for (int b = 0; b < n; ++b) rows = std::max(rows, dec_attn_chunk_rows(lens[b]));
+    g.box_rows = kDecAttnRaggedBox;
+    g.chunk_rows = (rows + kDecAttnRaggedBox - 1) / kDecAttnRaggedBox * kDecAttnRaggedBox;
+  }
+  g.smem = static_cast<size_t>(4) * g.chunk_rows * 128 + 128;
+  int per_sm = static_cast<int>((227 * 1024) / (g.smem + 8 * 1024));
+  per_sm = std::max(1, std::min(per_sm, 4));
+  g.grid = std::min(items, per_sm * num_sms);
+  return g;
+}
+
+template <int NQ, bool kPipe, bool kRagged>
+static int launch_decode_attn_inst(gitb200_engine* h, const DecAttnParams& ap, int grid, size_t smem, bool pdl,
+                                   cudaStream_t st, const CUtensorMap& tk, const CUtensorMap& tv) {
+  static size_t attr_done[64] = {0};
+  if (attr_done[h->device & 63] < smem) {
+    CK(cudaFuncSetAttribute(decode_attn_kernel<NQ, kPipe, kRagged>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+    attr_done[h->device & 63] = smem;
+  }
+  CK(launch_k(pdl, decode_attn_kernel<NQ, kPipe, kRagged>, dim3(grid), dim3(128), smem, st, tk, tv, ap));
+  CKL(h, "decode_attn_kernel");
+  return 0;
+}
+// decode_attn_kernel<beam, beam == 1, ragged> on `grid` CTAs; ap.chunk_rows / box_rows and smem from dec_attn_geometry.
+static int launch_decode_attn(gitb200_engine* h, const DecAttnParams& ap, int beam, int grid, size_t smem, bool pdl,
+                              cudaStream_t st) {
+  CUtensorMap tk, tv;
+  TRY(get_tmap(h, ap.img_k, static_cast<long long>(ap.B) * ap.M, ap.D, ap.D, ap.box_rows, &tk, false));
+  TRY(get_tmap(h, ap.img_v, static_cast<long long>(ap.B) * ap.M, ap.D, ap.D, ap.box_rows, &tv, false));
+  const bool rg = ap.img_lens != nullptr;
+  switch (beam) {
+    case 1: return rg ? launch_decode_attn_inst<1, true, true>(h, ap, grid, smem, pdl, st, tk, tv)
+                      : launch_decode_attn_inst<1, true, false>(h, ap, grid, smem, pdl, st, tk, tv);
+    case 2: return rg ? launch_decode_attn_inst<2, false, true>(h, ap, grid, smem, pdl, st, tk, tv)
+                      : launch_decode_attn_inst<2, false, false>(h, ap, grid, smem, pdl, st, tk, tv);
+    case 3: return rg ? launch_decode_attn_inst<3, false, true>(h, ap, grid, smem, pdl, st, tk, tv)
+                      : launch_decode_attn_inst<3, false, false>(h, ap, grid, smem, pdl, st, tk, tv);
+    case 4: return rg ? launch_decode_attn_inst<4, false, true>(h, ap, grid, smem, pdl, st, tk, tv)
+                      : launch_decode_attn_inst<4, false, false>(h, ap, grid, smem, pdl, st, tk, tv);
+    default: return fail(h, "decode: beam size %d not supported (1 .. 4)", beam);
+  }
+}
+
+// decode_attn_f32_kernel (parity mode): one warp per (sequence, head); *ctas receives the grid.
+static int launch_decode_attn_f32(gitb200_engine* h, const DecAttnF32Params& ap, bool pdl, cudaStream_t st, unsigned int* ctas) {
+  const size_t smem = static_cast<size_t>(4) * (192 + ap.M + ap.T_alloc) * sizeof(float);
+  if (smem > 200 * 1024) return fail(h, "parity decode attention: %d keys do not fit in shared memory", ap.M + ap.T_alloc);
+  CK(cudaFuncSetAttribute(decode_attn_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  *ctas = static_cast<unsigned int>((ap.R * (ap.D / 64) + 3) / 4);
+  CK(launch_k(pdl, decode_attn_f32_kernel, dim3(*ctas), dim3(128), smem, st, ap));
+  CKL(h, "decode_attn_f32_kernel");
   return 0;
 }
 
@@ -1271,12 +1341,8 @@ static int step_layers(gitb200_engine* h, Lane& ln_, const long long* tokens, co
       ap.state = state;
       ap.chain = cs;
       ap.img_lens = h->cur_ragged ? h->rg_lens.as<int>() : nullptr;
-      const size_t smem = static_cast<size_t>(4) * (192 + h->cur_M + h->T_alloc) * sizeof(float);
-      if (smem > 200 * 1024) return fail(h, "parity decode attention: %d keys do not fit in shared memory", h->cur_M + h->T_alloc);
-      CK(cudaFuncSetAttribute(decode_attn_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-      const unsigned int grid = static_cast<unsigned int>((R * h->cfg.dec_heads + 3) / 4);
-      CK(launch_k(pdl, decode_attn_f32_kernel, dim3(grid), dim3(128), smem, st, ap));
-      CKL(h, "decode_attn_f32_kernel");
+      unsigned int grid = 0;
+      TRY(launch_decode_attn_f32(h, ap, pdl, st, &grid));
       next_link(grid);
     } else {
       DecAttnParams ap{};
@@ -1289,23 +1355,9 @@ static int step_layers(gitb200_engine* h, Lane& ln_, const long long* tokens, co
       ap.chunk_rows = h->attn_chunk_rows; ap.box_rows = h->attn_box_rows;
       ap.chain = cs;
       ap.img_lens = h->cur_ragged ? h->rg_lens.as<int>() : nullptr;
-      CUtensorMap tk, tv;
-      TRY(get_tmap(h, ap.img_k, static_cast<long long>(ln_.nb) * h->cur_M, D, D, ap.box_rows, &tk, false));
-      TRY(get_tmap(h, ap.img_v, static_cast<long long>(ln_.nb) * h->cur_M, D, D, ap.box_rows, &tv, false));
-      dim3 grid(std::min(h->attn_grid, ln_.nb * h->cfg.dec_heads));
-      if (h->cur_ragged) {
-        if (beam == 1) CK(launch_k(pdl, decode_attn_kernel<1, true, true>, grid, dim3(128), h->attn_smem, st, tk, tv, ap));
-        else if (beam == 4) CK(launch_k(pdl, decode_attn_kernel<4, false, true>, grid, dim3(128), h->attn_smem, st, tk, tv, ap));
-        else if (beam == 3) CK(launch_k(pdl, decode_attn_kernel<3, false, true>, grid, dim3(128), h->attn_smem, st, tk, tv, ap));
-        else if (beam == 2) CK(launch_k(pdl, decode_attn_kernel<2, false, true>, grid, dim3(128), h->attn_smem, st, tk, tv, ap));
-        else return fail(h, "decode: beam size %d not supported (1 .. 4)", beam);
-      } else if (beam == 1) CK(launch_k(pdl, decode_attn_kernel<1, true>, grid, dim3(128), h->attn_smem, st, tk, tv, ap));
-      else if (beam == 4) CK(launch_k(pdl, decode_attn_kernel<4>, grid, dim3(128), h->attn_smem, st, tk, tv, ap));
-      else if (beam == 3) CK(launch_k(pdl, decode_attn_kernel<3>, grid, dim3(128), h->attn_smem, st, tk, tv, ap));
-      else if (beam == 2) CK(launch_k(pdl, decode_attn_kernel<2>, grid, dim3(128), h->attn_smem, st, tk, tv, ap));
-      else return fail(h, "decode: beam size %d not supported (1 .. 4)", beam);
-      CKL(h, "decode_attn_kernel");
-      next_link(grid.x);
+      const int grid = std::min(h->attn_grid, ln_.nb * h->cfg.dec_heads);
+      TRY(launch_decode_attn(h, ap, beam, grid, h->attn_smem, pdl, st));
+      next_link(static_cast<unsigned int>(grid));
     }
     TRY(skinny(gemm_skinny(ctx, D * ks, l.wo.as<bf16>(), D * ks, R, D, D * ks, nullptr, ACT_NONE, t, D, false, kOutProjSplits, skip, pdl)));
     TRY(ln(ln_partials(t, kOutProjSplits, R, l.bo.as<float>(), xd, l.lnag.as<float>(), l.lnab.as<float>(), xd, hd)));
@@ -1324,38 +1376,14 @@ static int step_layers(gitb200_engine* h, Lane& ln_, const long long* tokens, co
   return 0;
 }
 
-// Geometry of the decode-attention staging buffer: the image K/V slice of one (image, head) is M rows of 128 B;
-// up to 512 rows are staged per round as 1-2 TMA boxes of <= 256 rows.
-static int set_attn_smem_limit(gitb200_engine* h) {
-  const int M = h->cur_M;
-  // chunks of at most 224 keys: two (K + V) staging buffers of one chunk per CTA, and at least two CTAs per SM (M = 257
-  // in one piece would be 131 KB per CTA = one 4-warp CTA per SM)
-  const int n_chunks = (M + 223) / 224;
-  h->attn_box_rows = (M + n_chunks - 1) / n_chunks;
-  h->attn_chunk_rows = h->attn_box_rows;
-  if (h->cur_ragged) {
-    // every image is chunked by its own key count (dec_attn_chunk_rows) and fetched in 32-row boxes: the staging buffer
-    // holds the longest chunk of the call rounded up to whole boxes
-    int rows = 0;
-    for (int Lb : h->cur_lens) rows = std::max(rows, dec_attn_chunk_rows(Lb));
-    h->attn_box_rows = kDecAttnRaggedBox;
-    h->attn_chunk_rows = (rows + kDecAttnRaggedBox - 1) / kDecAttnRaggedBox * kDecAttnRaggedBox;
-  }
-  h->attn_smem = static_cast<size_t>(4) * h->attn_chunk_rows * 128 + 128;
-  int per_sm = static_cast<int>((227 * 1024) / (h->attn_smem + 8 * 1024));
-  per_sm = std::max(1, std::min(per_sm, 4));
-  const int items = h->cur_B * h->cfg.dec_heads;
-  h->attn_grid = std::min(items, per_sm * h->num_sms);
-  CK(cudaFuncSetAttribute(decode_attn_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(h->attn_smem)));
-  CK(cudaFuncSetAttribute(decode_attn_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(h->attn_smem)));
-  CK(cudaFuncSetAttribute(decode_attn_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(h->attn_smem)));
-  CK(cudaFuncSetAttribute(decode_attn_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(h->attn_smem)));
-  if (h->cur_ragged) {
-    CK(cudaFuncSetAttribute(decode_attn_kernel<1, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(h->attn_smem)));
-    CK(cudaFuncSetAttribute(decode_attn_kernel<4, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(h->attn_smem)));
-    CK(cudaFuncSetAttribute(decode_attn_kernel<3, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(h->attn_smem)));
-    CK(cudaFuncSetAttribute(decode_attn_kernel<2, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(h->attn_smem)));
-  }
+// Decode-attention geometry of the last prefill (dec_attn_geometry) and the step chain's counters.
+static int set_decode_geometry(gitb200_engine* h) {
+  const DecAttnGeom g = dec_attn_geometry(h->cur_M, h->cur_ragged ? h->cur_lens.data() : nullptr, h->cur_B, h->num_sms,
+                                          h->cur_B * h->cfg.dec_heads);
+  h->attn_chunk_rows = g.chunk_rows;
+  h->attn_box_rows = g.box_rows;
+  h->attn_smem = g.smem;
+  h->attn_grid = g.grid;
   CK(h->chain.ensure(256));
   CK(cudaMemset(h->chain.p, 0, 256));
   return 0;

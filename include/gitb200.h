@@ -62,7 +62,7 @@ enum { GITB200_F32 = 0, GITB200_BF16 = 1, GITB200_I64 = 2 };
 int gitb200_create(const gitb200_config* cfg, int device, gitb200_engine** out);
 void gitb200_destroy(gitb200_engine* h);
 const char* gitb200_last_error(const gitb200_engine* h);
-/* ABI version of the library (bumped on any signature change). */
+/* ABI version of the library (bumped on any signature change): 8 (gitb200_op_attention_ex, gitb200_op_decode_attention). */
 int gitb200_abi_version(void);
 
 /* Replaces: torch_common.load_state_dict -> module parameters           torch_common.py:93-145.
@@ -211,6 +211,26 @@ int gitb200_op_attention(const void* q_dev, const void* k_dev, const void* v_dev
                          long long q_row_stride, long long kv_row_stride, long long q_batch_stride,
                          long long kv_batch_stride, long long out_row_stride, long long out_batch_stride,
                          void* stream);
+/* gitb200_op_attention plus per-batch lengths and parity mode.  seq_lens_host: NULL or B lengths in 1..S (ragged: batches
+ * must be stored back to back; batch b is computed as a call with S = seq_lens[b] and its rows past that length are
+ * zeros).  fp32 != 0: attn_f32_kernel on fp32 q/k/v; output rows are 3*H*64 bf16 [hi | lo | hi], out_row_stride is
+ * ignored. */
+int gitb200_op_attention_ex(const void* q_dev, const void* k_dev, const void* v_dev, void* out_dev, int B, int S, int H,
+                            long long q_row_stride, long long kv_row_stride, long long q_batch_stride,
+                            long long kv_batch_stride, long long out_row_stride, long long out_batch_stride,
+                            const int32_t* seq_lens_host, int fp32, void* stream);
+/* One layer's decode-step attention as the kernel chain runs it: decode_attn_kernel<beam, beam == 1, img_lens != NULL>,
+ * or decode_attn_f32_kernel when fp32 != 0.
+ * qkv_dev: n_partials (1..4) fp32 split-K partial buffers [B*beam, 3*D], B*beam*3*D elements apart; bqkv_dev fp32 [3*D].
+ * img_k/v_dev [B, M, D] and txt_k/v_dev [B*beam, T_alloc, D]: bf16, or fp32 when fp32 != 0.  Position pos of every text
+ * row is written (k / v of this step + bias).  src_row_dev int32 [B*beam, T_alloc] or NULL (identity).
+ * img_lens_host: NULL (uniform) or B key counts in 1..M (ragged).  ctx_dev: bf16 [B*beam, D], or split rows [B*beam, 3*D]
+ * when fp32 != 0.  grid: CTAs of decode_attn_kernel in 0..B*D/64, 0 = what the engine would launch (ignored when
+ * fp32 != 0).  beam 1..4, D % 64 == 0. */
+int gitb200_op_decode_attention(const float* qkv_dev, int n_partials, const float* bqkv_dev, const void* img_k_dev,
+                                const void* img_v_dev, void* txt_k_dev, void* txt_v_dev, const int32_t* src_row_dev,
+                                void* ctx_dev, int B, int beam, int M, const int32_t* img_lens_host, int T_alloc, int pos,
+                                int D, int fp32, int grid, void* stream);
 
 /* ---- test-time image transform on the GPU ----------------------------------------------------------------
  * Replaces: get_image_transform(param)(pil_image)                                       inference.py:111-132

@@ -152,4 +152,5 @@ def test_flash_attention(B, S, H):
     k = k.view(B, S, H, 64).transpose(1, 2)
     v = v.view(B, S, H, 64).transpose(1, 2)
     ref = (torch.softmax(q @ k.transpose(-1, -2) / 8.0, dim=-1) @ v).transpose(1, 2).reshape(B, S, d)
-    assert (out.float() - ref).abs().max().item() < 2e-2
+    # the flash_attn_wgmma_kernel bound of tests/test_gpu_attention.py
+    assert (out.float() - ref).abs().max().item() <= 3.5e-3 * v.abs().max().item() + 1e-5
