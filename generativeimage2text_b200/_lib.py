@@ -5,7 +5,7 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, 'libgitb200.so')
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 c_void_p, c_int, c_int64, c_float, c_char_p = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_char_p
 c_ll = ctypes.c_longlong
@@ -79,6 +79,11 @@ SIGNATURES = {
                                      c_ll, c_ll, c_void_p]),
     'gitb200_op_attention_ex': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_ll, c_ll, c_ll,
                                         c_ll, c_ll, c_ll, ctypes.POINTER(ctypes.c_int32), c_int, c_void_p]),
+    'gitb200_score': (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p,
+                               c_void_p, c_void_p]),
+    'gitb200_op_text_attention': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int,
+                                          c_int, ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int32), c_int, c_int,
+                                          c_void_p]),
     'gitb200_op_decode_attention': (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                             c_void_p, c_int, c_int, c_int, ctypes.POINTER(ctypes.c_int32), c_int, c_int,
                                             c_int, c_int, c_int, c_void_p]),

@@ -321,6 +321,160 @@ __global__ void __launch_bounds__(128) flash_attn_wgmma_kernel(const __grid_cons
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// text_attn_wgmma_kernel: the text rows of a whole caption batch in one pass (caption scoring, the training-branch forward
+// of reference layers/decoder.py:916-972 through BertEncoderAsDecoder's block mask :114-137).  Text row t of caption n
+// attends to the M_b image keys of its image (image_index[n]) and to text keys 0..t of its own caption.
+//   One CTA = one warpgroup per (64 text query rows, head, caption), exactly the arithmetic of flash_attn_wgmma_kernel:
+//   the image keys come first as 64-key blocks of the image K/V cache (masked past M_b), then the caption's own text
+//   K/V blocks 0 .. q0 / 64, with the causal mask on the diagonal block only.  Text blocks past the query tile are never
+//   loaded.  A sibling of flash_attn_wgmma_kernel (same smem ring, same block step) so that kernel's code is untouched.
+// ------------------------------------------------------------------------------------------------
+struct TextAttnParams {
+  __nv_bfloat16* out;          // [N * T] rows of H * 64, row stride o_rs
+  int N, T, H;                 // captions, positions per caption, heads
+  int M;                       // rows per image in the image K/V view (slot length)
+  const int* img_lens;         // null, or [B] valid image keys of each image (ragged batches; <= M)
+  const int* image_index;      // null (caption n uses image n), or [N]
+  long long o_rs;
+  float scale_log2;            // (1/sqrt(64)) * log2(e)
+};
+
+__global__ void __launch_bounds__(128) text_attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ,
+                                                             const __grid_constant__ CUtensorMap tmK,
+                                                             const __grid_constant__ CUtensorMap tmV,
+                                                             const __grid_constant__ CUtensorMap tmIK,
+                                                             const __grid_constant__ CUtensorMap tmIV,
+                                                             const TextAttnParams p) {
+  extern __shared__ __align__(1024) uint8_t attn_smem_raw[];
+  uint8_t* smem = attn_smem_raw + ((1024u - (smem_u32(attn_smem_raw) & 1023u)) & 1023u);
+  uint8_t* sQ = smem;
+  uint8_t* sK = smem + 8192;                     // [2 stages][64 keys][128 B]
+  uint8_t* sV = smem + 3 * 8192;
+  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 5 * 8192);   // [0] Q, [1 + stage] K | V
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int h = blockIdx.y, n = blockIdx.z;
+  const int q0 = blockIdx.x * kAttnWgRows;
+  const int img = p.image_index != nullptr ? p.image_index[n] : n;
+  const int Mb = p.img_lens != nullptr ? p.img_lens[img] : p.M;
+  const int n_img = (Mb + kAttnWgRows - 1) / kAttnWgRows;
+  const int nblk = n_img + q0 / kAttnWgRows + 1;  // image blocks, then text blocks 0 .. the diagonal one
+  const int trow = n * p.T;                      // rows of caption n in the [N * T, H * 64] q / k / v views
+  auto load_kv = [&](int blk, int st) {
+    mbar_arrive_expect_tx(&bar[1 + st], 2 * 8192);
+    if (blk < n_img) {
+      tma_load_2d(sK + st * 8192, &tmIK, &bar[1 + st], h * 64, img * p.M + blk * kAttnWgRows);
+      tma_load_2d(sV + st * 8192, &tmIV, &bar[1 + st], h * 64, img * p.M + blk * kAttnWgRows);
+    } else {
+      tma_load_2d(sK + st * 8192, &tmK, &bar[1 + st], h * 64, trow + (blk - n_img) * kAttnWgRows);
+      tma_load_2d(sV + st * 8192, &tmV, &bar[1 + st], h * 64, trow + (blk - n_img) * kAttnWgRows);
+    }
+  };
+  if (tid == 0) {
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmK);
+    tma_prefetch_desc(&tmV);
+    tma_prefetch_desc(&tmIK);
+    tma_prefetch_desc(&tmIV);
+    for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1);
+    mbar_fence_init();
+  }
+  __syncthreads();
+  if (tid == 0) {
+    mbar_arrive_expect_tx(&bar[0], 8192);
+    tma_load_2d(sQ, &tmQ, &bar[0], h * 64, trow + q0);
+    load_kv(0, 0);
+    if (nblk > 1) load_kv(1, 1);
+  }
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  const int g0 = warp * 16 + (lane >> 2);        // tile rows of registers e < 2 (g0) and e >= 2 (g0 + 8)
+  mbar_wait(&bar[0], 0);
+  for (int blk = 0; blk < nblk; ++blk) {
+    const int st = blk & 1;
+    mbar_wait(&bar[1 + st], (blk >> 1) & 1);
+    float s[32];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      Wgmma<64>::mma(s, wgmma_desc_sw128(smem_u32(sQ) + k * 32), wgmma_desc_sw128(smem_u32(sK + st * 8192) + k * 32), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    // register 4j + e: row g0 (e < 2) or g0 + 8 (e >= 2), key (of this block) 8j + 2 (lane % 4) + (e & 1)
+    const int kk0 = 2 * (lane & 3);
+    float mx[2] = {-INFINITY, -INFINITY};
+    if (blk < n_img) {                           // image keys: those past M_b are masked
+      const int lim = Mb - blk * kAttnWgRows;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int kk = kk0 + 8 * j;
+        if (kk >= lim) { s[4 * j] = -INFINITY; s[4 * j + 2] = -INFINITY; }
+        if (kk + 1 >= lim) { s[4 * j + 1] = -INFINITY; s[4 * j + 3] = -INFINITY; }
+      }
+    } else if (blk + 1 == nblk) {                // the diagonal text block: key q0 + kk is visible to row q0 + r iff kk <= r
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int kk = kk0 + 8 * j;
+        if (kk > g0) s[4 * j] = -INFINITY;
+        if (kk + 1 > g0) s[4 * j + 1] = -INFINITY;
+        if (kk > g0 + 8) s[4 * j + 2] = -INFINITY;
+        if (kk + 1 > g0 + 8) s[4 * j + 3] = -INFINITY;
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      mx[0] = fmaxf(mx[0], fmaxf(s[4 * j], s[4 * j + 1]));
+      mx[1] = fmaxf(mx[1], fmaxf(s[4 * j + 2], s[4 * j + 3]));
+    }
+    float corr[2], m_new[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
+      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
+      m_new[i] = fmaxf(m_run[i], mx[i]);         // finite: every block holds at least one visible key for every row
+      corr[i] = exp2f((m_run[i] - m_new[i]) * p.scale_log2);
+      m_run[i] = m_new[i];
+      l_run[i] *= corr[i];
+    }
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const uint32_t lo = pack_bf16(exp2f((s[4 * j] - m_new[0]) * p.scale_log2), exp2f((s[4 * j + 1] - m_new[0]) * p.scale_log2));
+      const uint32_t hi = pack_bf16(exp2f((s[4 * j + 2] - m_new[1]) * p.scale_log2), exp2f((s[4 * j + 3] - m_new[1]) * p.scale_log2));
+      l_run[0] += bf16_lo(lo) + bf16_hi(lo);
+      l_run[1] += bf16_lo(hi) + bf16_hi(hi);
+      pa[j >> 1][(j & 1) * 2 + 0] = lo;
+      pa[j >> 1][(j & 1) * 2 + 1] = hi;
+      o[4 * j] *= corr[0];
+      o[4 * j + 1] *= corr[0];
+      o[4 * j + 2] *= corr[1];
+      o[4 * j + 3] *= corr[1];
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_rs_mn(o, pa[kk], wgmma_desc_sw128(smem_u32(sV + st * 8192) + kk * 2048));
+    wgmma_commit();
+    wgmma_wait<0>();
+    __syncthreads();                             // every warp is done with stage st: refill it with block blk + 2
+    if (tid == 0 && blk + 2 < nblk) load_kv(blk + 2, st);
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    l_run[i] += __shfl_xor_sync(0xffffffffu, l_run[i], 1);
+    l_run[i] += __shfl_xor_sync(0xffffffffu, l_run[i], 2);
+  }
+  const float inv0 = 1.0f / l_run[0], inv1 = 1.0f / l_run[1];
+  const int r0 = q0 + g0, r1 = r0 + 8;
+  __nv_bfloat16* og = p.out + static_cast<long long>(trow) * p.o_rs + h * 64 + 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    if (r0 < p.T) *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r0) * p.o_rs + 8 * j) = pack_bf16(o[4 * j] * inv0, o[4 * j + 1] * inv0);
+    if (r1 < p.T) *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r1) * p.o_rs + 8 * j) = pack_bf16(o[4 * j + 2] * inv1, o[4 * j + 3] * inv1);
+  }
+}
+
 // one MUFU.EX2 (exp2f() adds a denormal-range fix-up the softmax does not need: those terms vanish against a row sum >= 1)
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
@@ -796,6 +950,77 @@ __global__ void __launch_bounds__(128) attn_f32_kernel(const AttnF32Params p) {
   }
   __nv_bfloat16* orow = p.out + b * p.o_bs + static_cast<long long>(row) * 3 * p.d_model;
   store_split3_pair(orow, p.d_model, h * 64 + 2 * lane, a0 / sum, a1 / sum);
+}
+
+// Parity-mode sibling of text_attn_wgmma_kernel: plain fp32, one warp per (caption, head, text row); q / k / v fp32 rows of
+// d_model elements ([N * T] text rows, [B * M] image rows), output rows in the split format [hi | lo | hi] (3 * d_model).
+struct TextAttnF32Params {
+  const float* q;
+  const float* k;                // text K / V [N * T, d_model]
+  const float* v;
+  const float* img_k;            // image K / V [B * M, d_model]
+  const float* img_v;
+  __nv_bfloat16* out;            // [N * T, 3 * d_model]
+  int N, T, H, d_model, M;
+  const int* img_lens;           // null or [B]
+  const int* image_index;        // null or [N]
+};
+
+__global__ void __launch_bounds__(128) text_attn_f32_kernel(const TextAttnF32Params p) {
+  extern __shared__ float attn_f32_smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* q_s = attn_f32_smem + warp * (64 + p.M + p.T);
+  float* sc = q_s + 64;
+  const long long item = static_cast<long long>(blockIdx.x) * 4 + warp;
+  const long long total = static_cast<long long>(p.N) * p.H * p.T;
+  if (item >= total) return;
+  const int t = static_cast<int>(item % p.T);
+  const int h = static_cast<int>((item / p.T) % p.H);
+  const int n = static_cast<int>(item / (static_cast<long long>(p.T) * p.H));
+  const int img = p.image_index != nullptr ? p.image_index[n] : n;
+  const int Mb = p.img_lens != nullptr ? p.img_lens[img] : p.M;
+  const int n_keys = Mb + t + 1;
+  const long long trow = static_cast<long long>(n) * p.T;
+  const float* qg = p.q + (trow + t) * p.d_model + h * 64;
+  auto key_row = [&](int j, bool want_v) -> const float* {
+    if (j < Mb) return (want_v ? p.img_v : p.img_k) + (static_cast<long long>(img) * p.M + j) * p.d_model + h * 64;
+    return (want_v ? p.v : p.k) + (trow + j - Mb) * p.d_model + h * 64;
+  };
+  q_s[lane] = qg[lane] * 0.125f;             // Q / sqrt(64) before the product (reference layers/bert/modeling_bert.py:42-43)
+  q_s[lane + 32] = qg[lane + 32] * 0.125f;
+  __syncwarp();
+  float mx = -INFINITY;
+  for (int j0 = 0; j0 < n_keys; j0 += 32) {
+    const int j = j0 + lane;
+    if (j < n_keys) {
+      const float4* kr = reinterpret_cast<const float4*>(key_row(j, false));
+      float a = 0.f;
+#pragma unroll
+      for (int d = 0; d < 16; ++d) {
+        const float4 kk = kr[d];
+        a = fmaf(q_s[4 * d], kk.x, a); a = fmaf(q_s[4 * d + 1], kk.y, a);
+        a = fmaf(q_s[4 * d + 2], kk.z, a); a = fmaf(q_s[4 * d + 3], kk.w, a);
+      }
+      sc[j] = a;
+      mx = fmaxf(mx, a);
+    }
+  }
+  mx = warp_max(mx);
+  float sum = 0.f;
+  for (int j = lane; j < n_keys; j += 32) {
+    const float e = expf(sc[j] - mx);
+    sc[j] = e;
+    sum += e;
+  }
+  sum = warp_sum(sum);
+  __syncwarp();
+  float a0 = 0.f, a1 = 0.f;
+  for (int j = 0; j < n_keys; ++j) {
+    const float2 vv = *reinterpret_cast<const float2*>(key_row(j, true) + 2 * lane);
+    a0 = fmaf(sc[j], vv.x, a0);
+    a1 = fmaf(sc[j], vv.y, a1);
+  }
+  store_split3_pair(p.out + (trow + t) * 3 * p.d_model, p.d_model, h * 64 + 2 * lane, a0 / sum, a1 / sum);
 }
 
 struct DecAttnF32Params {

@@ -42,11 +42,17 @@ struct GemmParams {
   int split3;                 // bf16 output in the parity mode's operand format: row = [hi | lo | hi] (3 x N columns, ldo = 3N)
   int pdl;                    // launched with programmatic dependent launch: prefetch weights, then griddep_wait()
   ChainSync chain;            // flag-based ordering inside the decode step (see ptx.cuh); counters == null: off
+  const int* lse_target;      // EPI_LSE: [M] target column of each row (-1: none); out[0] = float4 partials [M][ldo]
 };
 
 // Epilogue variants are compile-time (the runtime-flag version spent ~700 warp instructions per 32x32 chunk,
 // which made every K=768 GEMM of the encoder epilogue-issue bound).
 constexpr int EPI_TRANSPOSED = 1, EPI_BF16 = 2, EPI_RESID = 4, EPI_PARTIAL = 8, EPI_ACT_SHIFT = 4, EPI_SPLIT3 = 64;
+// EPI_LSE (normal shape, fp32, caption scoring's LM head): no logits are stored.  Each MMA warp folds the columns it owns of
+// a tile (BN / 2 of them: 32 of every 64-column chunk) into per-row statistics (max, sum exp(x - max), sum x, x[target])
+// and stores them as one float4 per (row, half tile) to out[0] + row * ldo + 2 * n_blk + half; lse_combine_kernel
+// (rowops.cuh) folds a row's partials in column order.
+constexpr int EPI_LSE = 128;
 constexpr int epi_code(bool transposed, bool bf16, bool resid, bool partial, int act) {
   return (transposed ? EPI_TRANSPOSED : 0) | (bf16 ? EPI_BF16 : 0) | (resid ? EPI_RESID : 0) | (partial ? EPI_PARTIAL : 0) |
          (act << EPI_ACT_SHIFT);
@@ -238,12 +244,52 @@ __device__ __forceinline__ void epi_store_transposed(const GemmParams& p, const 
   }
 }
 
+// EPI_LSE: fold one 32 x 32 chunk staged as [row][column] (see epi_store_normal) into the running statistics of the lane's
+// 8 rows (row0 + it * 4 + lane / 8) over its 4 columns n0 + 4 (lane % 8) ..; columns >= N do not exist.
+__device__ __forceinline__ void epi_lse_accum(const GemmParams& p, const uint8_t* stg, int lane, int n0, const int (&tgt)[8],
+                                              float (&m)[8], float (&se)[8], float (&sx)[8], float (&xt)[8]) {
+  const int c4 = lane & 7;
+  const int rsub = lane >> 3;
+  const int col0 = n0 + c4 * 4;
+  float b[4];
+  bool ok[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    ok[e] = col0 + e < p.N;
+    b[e] = ok[e] ? __ldg(p.bias + col0 + e) : 0.f;
+  }
+#pragma unroll
+  for (int it = 0; it < 8; ++it) {
+    const int rr = it * 4 + rsub;
+    const float4 v = *reinterpret_cast<const float4*>(stg + rr * 128 + ((c4 ^ (rr & 7)) << 4));
+    const float x[4] = {v.x + b[0], v.y + b[1], v.z + b[2], v.w + b[3]};
+    float cm = -INFINITY;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) if (ok[e]) cm = fmaxf(cm, x[e]);
+    const float nm = fmaxf(m[it], cm);
+    if (nm == -INFINITY) continue;               // no column of this chunk exists
+    float acc = (m[it] == -INFINITY) ? 0.f : se[it] * __expf(m[it] - nm);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      if (ok[e]) {
+        acc += __expf(x[e] - nm);
+        sx[it] += x[e];
+        if (tgt[it] == col0 + e) xt[it] = x[e];
+      }
+    }
+    se[it] = acc;
+    m[it] = nm;
+  }
+}
+
 template <int BN, int EPI>
 __global__ void __launch_bounds__(GemmCfg<BN>::THREADS, 1)
 gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const GemmParams p) {
   using C = GemmCfg<BN>;
   constexpr bool kTransposed = (EPI & EPI_TRANSPOSED) != 0;
+  constexpr bool kLse = (EPI & EPI_LSE) != 0;
+  static_assert(!kLse || EPI == EPI_LSE, "the statistics epilogue takes no other option");
   if (p.pdl) griddep_launch_early();
   if (p.pdl) tl_mark(100000 + 1000 + static_cast<int>(gridDim.x));
   // `skip` (decode finished) only changes between steps, which are separated by full dependencies
@@ -377,7 +423,17 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       const int row0 = m_blk * C::BM + mw * 64 + (warp & 1) * 32;   // first tile row of this warp's block
       long long ooff[8];
       uint32_t okmask = 0;
-      if (!kTransposed) okmask = epi_row_offsets(p, row0, rsub, store_ok, ooff);
+      if (!kTransposed && !kLse) okmask = epi_row_offsets(p, row0, rsub, store_ok, ooff);
+      float lm[8], lse_s[8], lsx[8], lxt[8];
+      int ltg[8];
+      if constexpr (kLse) {
+#pragma unroll
+        for (int it = 0; it < 8; ++it) {
+          const int row = row0 + it * 4 + rsub;
+          ltg[it] = row < p.M ? p.lse_target[row] : -1;
+          lm[it] = -INFINITY; lse_s[it] = 0.f; lsx[it] = 0.f; lxt[it] = 0.f;
+        }
+      }
 #pragma unroll
       for (int cc = 0; cc < BN / 64; ++cc) {
         if (n_blk * BN + cc * 64 >= p.N) break;   // uniform over the warpgroup
@@ -400,12 +456,36 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         }
         named_bar_sync(1 + mw, 128);
         const int n0 = n_blk * BN + cc * 64 + (warp >> 1) * 32;
-        if (!kTransposed) {
+        if constexpr (kLse) {
+          epi_lse_accum(p, stg, lane, n0, ltg, lm, lse_s, lsx, lxt);
+        } else if (!kTransposed) {
           if (n0 < p.N) epi_store_normal<EPI>(p, stg, lane, n0, row0, ooff, okmask);
         } else {
           epi_store_transposed<EPI>(p, stg, lane, n0, row0, split, store_ok);
         }
         named_bar_sync(1 + mw, 128);   // the staging buffer is rewritten by the next chunk
+      }
+      if constexpr (kLse) {
+        // the 8 lanes of a row merge their statistics (butterfly: every lane ends with the same values), lane 0 stores
+#pragma unroll
+        for (int it = 0; it < 8; ++it) {
+#pragma unroll
+          for (int o = 1; o < 8; o <<= 1) {
+            const float m_o = __shfl_xor_sync(0xffffffffu, lm[it], o);
+            const float s_o = __shfl_xor_sync(0xffffffffu, lse_s[it], o);
+            const float nm = fmaxf(lm[it], m_o);
+            const float sa = (lm[it] == -INFINITY) ? 0.f : lse_s[it] * __expf(lm[it] - nm);
+            const float sb = (m_o == -INFINITY) ? 0.f : s_o * __expf(m_o - nm);
+            lse_s[it] = sa + sb;
+            lm[it] = nm;
+            lsx[it] += __shfl_xor_sync(0xffffffffu, lsx[it], o);
+            lxt[it] += __shfl_xor_sync(0xffffffffu, lxt[it], o);
+          }
+          const int row = row0 + it * 4 + rsub;
+          if ((lane & 7) == 0 && row < p.M)
+            reinterpret_cast<float4*>(p.out[0])[static_cast<long long>(row) * p.ldo + 2 * n_blk + (warp >> 1)] =
+                make_float4(lm[it], lse_s[it], lsx[it], lxt[it]);
+        }
       }
     }
   }

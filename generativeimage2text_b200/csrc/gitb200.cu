@@ -13,6 +13,8 @@
 //                  padding rows hold finite values that no valid row reads.
 //   text K/V     : bf16 [layer][k|v][rows][T_alloc][768] + int32 src_row[rows][T_alloc] indirection for beams.
 //   decode step  : fp32 row state [rows, 768], bf16 copy for the GEMMs, fp32 qkv / logits.
+//   scoring      : the text rows of N captions x T positions as [N * T, 768] row blocks (one layer's text K/V at a time);
+//                  no logits: LM-head statistics [N * T][2 * column tiles] float4 (gemm.cuh EPI_LSE).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -41,7 +43,7 @@
 using namespace gitb200;
 typedef __nv_bfloat16 bf16;
 
-#define GITB200_ABI_VERSION 8
+#define GITB200_ABI_VERSION 9
 
 // ------------------------------------------------------------------------------------------------
 // errors
@@ -154,6 +156,8 @@ struct gitb200_engine {
   DevBuf y_t, qb_t, mega_bar;                               // decode_mega_kernel: pre-LN sums, bf16 q, grid-barrier counters
   DevBuf state, next_token, logprob_sum, tokens_i64, stage_img, stage_tok, stage_lp, prefix_dev;
   DevBuf beam_ws;                                           // beam-search bookkeeping (search.cuh)
+  DevBuf sc_t, sc_x, sc_h, sc_q, sc_kv, sc_ctx, sc_u;       // caption scoring: text-row workspaces (score_impl)
+  DevBuf sc_tgt, sc_part, sc_loss, sc_valid, sc_index;      // ... LM-head targets / statistics, per-row losses, op image_index
   DevBuf sel_ws;                                            // greedy selection partials
   DevBuf chain;                                             // decode-step kernel chain completion counters [64]
   int attn_chunk_rows = 0, attn_box_rows = 0, attn_grid = 0;
@@ -334,6 +338,10 @@ static int launch_gemm_inst(gitb200_engine* h, const GemmCall& c, cudaStream_t s
 template <int BN>
 static int launch_gemm_bn(gitb200_engine* h, const GemmCall& c, cudaStream_t st) {
   const GemmParams& p = c.p;
+  if constexpr (BN == 256) {   // caption scoring's LM head: statistics only (see EPI_LSE)
+    if (p.lse_target != nullptr) return launch_gemm_inst<BN, EPI_LSE>(h, c, st);
+  }
+  if (p.lse_target != nullptr) return fail(h, "gemm: the LM-head statistics epilogue runs with 256-column tiles only");
   const int code = epi_code(p.transposed != 0, p.out_bf16 != 0, p.resid != nullptr, p.partial != 0, p.act) | (p.split3 ? EPI_SPLIT3 : 0);
   if constexpr (BN == 256) {   // parity mode: bf16 outputs that feed another GEMM leave as [hi | lo | hi]
     switch (code) {
@@ -394,13 +402,13 @@ static int launch_gemm(gitb200_engine* h, GemmCall c, cudaStream_t st) {
     p.rows_per_batch = p.M;
     p.batch_stride = p.M;
   }
-  if (!p.transposed && (p.N % 32 != 0 || p.seg_n % 32 != 0))
+  if (!p.transposed && p.lse_target == nullptr && (p.N % 32 != 0 || p.seg_n % 32 != 0))
     return fail(h, "gemm: N and segment width must be multiples of 32 (N=%d seg=%d)", p.N, p.seg_n);
   if (p.partial && !p.transposed) return fail(h, "gemm: split-K partial buffers are only implemented for the transposed epilogue");
   if (p.k_splits > 1 && !p.partial) return fail(h, "gemm: k_splits > 1 needs the partial-sum epilogue");
   if (p.partial && p.split_stride < static_cast<long long>(p.N) * p.ldo) return fail(h, "gemm: split_stride smaller than one partial buffer");
   int bn = c.bn > 0 ? c.bn : pick_bn(h, p.M, p.N, p.transposed != 0);
-  if (p.split3 && !p.transposed) bn = 256;
+  if ((p.split3 || p.lse_target != nullptr) && !p.transposed) bn = 256;
   switch (bn) {
     case 64: return launch_gemm_bn<64>(h, c, st);
     case 128: return launch_gemm_bn<128>(h, c, st);
@@ -517,6 +525,39 @@ static int launch_attention_f32(gitb200_engine* h, const AttnF32Params& p, cudaS
   const long long items = static_cast<long long>(p.B) * p.H * p.S;
   attn_f32_kernel<<<static_cast<unsigned int>((items + 3) / 4), 128, smem, st>>>(p);
   CKL(h, "attn_f32_kernel");
+  return 0;
+}
+
+// Caption scoring's text rows (attention.cuh text_attn_wgmma_kernel): q / k / v [N * T, H * 64] back to back, image K / V
+// [B * M, H * 64]; out rows o_rs apart.
+static int launch_text_attention(gitb200_engine* h, const bf16* q, const bf16* k, const bf16* v, const bf16* img_k,
+                                 const bf16* img_v, int B, const TextAttnParams& ap, cudaStream_t st) {
+  TextAttnParams p = ap;
+  p.scale_log2 = 0.125f * 1.44269504088896340736f;
+  const long long rows = static_cast<long long>(ap.N) * ap.T, irows = static_cast<long long>(B) * ap.M, cols = ap.H * 64;
+  CUtensorMap tq, tk, tv, tik, tiv;
+  TRY(get_tmap(h, q, rows, cols, cols, kAttnWgRows, &tq));
+  TRY(get_tmap(h, k, rows, cols, cols, kAttnWgRows, &tk));
+  TRY(get_tmap(h, v, rows, cols, cols, kAttnWgRows, &tv));
+  TRY(get_tmap(h, img_k, irows, cols, cols, kAttnWgRows, &tik));
+  TRY(get_tmap(h, img_v, irows, cols, cols, kAttnWgRows, &tiv));
+  const dim3 grid((ap.T + kAttnWgRows - 1) / kAttnWgRows, ap.H, ap.N);
+  text_attn_wgmma_kernel<<<grid, 128, kAttnWgSmem, st>>>(tq, tk, tv, tik, tiv, p);
+  CKL(h, "text_attn_wgmma_kernel");
+  return 0;
+}
+
+static int launch_text_attention_f32(gitb200_engine* h, const TextAttnF32Params& p, cudaStream_t st) {
+  const size_t smem = static_cast<size_t>(4) * (64 + p.M + p.T) * sizeof(float);
+  if (smem > 200 * 1024) return fail(h, "parity text attention: %d keys do not fit in shared memory", p.M + p.T);
+  static size_t attr_done[64] = {0};
+  if (attr_done[h->device & 63] < smem) {
+    CK(cudaFuncSetAttribute(text_attn_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+    attr_done[h->device & 63] = smem;
+  }
+  const long long items = static_cast<long long>(p.N) * p.H * p.T;
+  text_attn_f32_kernel<<<static_cast<unsigned int>((items + 3) / 4), 128, smem, st>>>(p);
+  CKL(h, "text_attn_f32_kernel");
   return 0;
 }
 
@@ -744,7 +785,9 @@ static void release_all(gitb200_engine* h) {
                     &h->pt, &h->pxd, &h->phd, &h->pq, &h->pctx, &h->pu, &h->img_kv, &h->txt_kv, &h->src_row[0],
                     &h->src_row[1], &h->xd_t, &h->hd_t, &h->qkv_t, &h->ctx_t, &h->t_t, &h->u_t, &h->logits, &h->state,
                     &h->next_token, &h->logprob_sum, &h->tokens_i64, &h->stage_img, &h->stage_tok, &h->stage_lp,
-                    &h->prefix_dev, &h->beam_ws, &h->sel_ws, &h->chain, &h->rg_tab, &h->rg_lens};
+                    &h->prefix_dev, &h->beam_ws, &h->sel_ws, &h->chain, &h->rg_tab, &h->rg_lens, &h->sc_t, &h->sc_x,
+                    &h->sc_h, &h->sc_q, &h->sc_kv, &h->sc_ctx, &h->sc_u, &h->sc_tgt, &h->sc_part, &h->sc_loss,
+                    &h->sc_valid, &h->sc_index};
   for (DevBuf* b : bufs) b->release();
   for (auto& l : h->enc) {
     DevBuf* lb[] = {&l.wqkv, &l.bqkv, &l.wo, &l.bo, &l.ln1g, &l.ln1b, &l.ln2g, &l.ln2b, &l.w1, &l.b1, &l.w2, &l.b2};
@@ -1177,13 +1220,11 @@ static char* txt_kv_ptr(gitb200_engine* h, int layer, int kv, long long elem_off
   return h->txt_kv.as<char>() + ((static_cast<long long>(layer) * 2 + kv) * per + elem_off) * h->kvb();
 }
 
-static int prefill_impl(gitb200_engine* h, int B, int beam, int T_alloc, float* vproj_out, cudaStream_t st) {
-  if (B != h->cur_B || h->cur_M <= 0) return fail(h, "prefill: call encode with the same batch first");
-  const int D = h->D, F = h->F, d = h->d, M = h->cur_M, nl = h->cfg.dec_layers, H = h->cfg.dec_heads;
-  const long long rows = static_cast<long long>(B) * M;
-  const int R = B * beam;
+// Workspaces of the image rows of the decoder (visual projection + layers) and the image K/V cache of the last encode.
+static int image_rows_buffers(gitb200_engine* h) {
+  const int D = h->D, F = h->F, nl = h->cfg.dec_layers;
+  const long long rows = static_cast<long long>(h->cur_B) * h->cur_M;
   const int ks = h->ks();
-  const bool par = h->parity;
   const long long kvb = static_cast<long long>(h->kvb());
   CK(h->pt.ensure(rows * D * 4));
   CK(h->pxd.ensure(rows * D * 4));
@@ -1192,6 +1233,17 @@ static int prefill_impl(gitb200_engine* h, int B, int beam, int T_alloc, float* 
   CK(h->pctx.ensure(rows * D * 2 * ks));
   CK(h->pu.ensure(rows * F * 2 * ks));
   CK(h->img_kv.ensure(static_cast<long long>(nl) * 2 * rows * D * kvb));
+  return 0;
+}
+static int image_rows(gitb200_engine* h, float* vproj_out, cudaStream_t st);
+
+static int prefill_impl(gitb200_engine* h, int B, int beam, int T_alloc, float* vproj_out, cudaStream_t st) {
+  if (B != h->cur_B || h->cur_M <= 0) return fail(h, "prefill: call encode with the same batch first");
+  const int D = h->D, F = h->F, nl = h->cfg.dec_layers;
+  const int R = B * beam;
+  const int ks = h->ks();
+  const long long kvb = static_cast<long long>(h->kvb());
+  TRY(image_rows_buffers(h));
   {
     // decode_mega_kernel fetches whole 64-position boxes of the text cache and masks the positions past the caption's end
     // by giving them probability 0 -- which only works if what lies there is finite: a fresh allocation is zeroed once
@@ -1218,6 +1270,17 @@ static int prefill_impl(gitb200_engine* h, int B, int beam, int T_alloc, float* 
   h->cur_beam = beam;
   h->cur_rows = R;
   h->T_alloc = T_alloc;
+  return image_rows(h, vproj_out, st);
+}
+
+// The image rows of the decoder, computed once per encode: visual projection, then the layers over the image rows only
+// (they never attend to text, reference layers/decoder.py:119-120), whose k / v rows fill the image K/V cache.  Buffers
+// from image_rows_buffers.
+static int image_rows(gitb200_engine* h, float* vproj_out, cudaStream_t st) {
+  const int D = h->D, F = h->F, d = h->d, M = h->cur_M, B = h->cur_B, nl = h->cfg.dec_layers, H = h->cfg.dec_heads;
+  const long long rows = static_cast<long long>(B) * M;
+  const int ks = h->ks();
+  const bool par = h->parity;
   float* t = h->pt.as<float>();
   float* xd = h->pxd.as<float>();
   bf16* hd = h->phd.as<bf16>();

@@ -443,6 +443,148 @@ embed_ln_kernel(const long long* __restrict__ tokens, long long tok_stride, cons
 }
 
 // ------------------------------------------------------------------------------------------------
+// Caption scoring (teacher-forced pass over whole captions, reference layers/decoder.py:916-972)
+// ------------------------------------------------------------------------------------------------
+// embed_ln_kernel for rows * T positions at once: row r holds token tokens[r] at position r % T.  Also writes the LM-head
+// target of each row, the next token of its caption (-1 for the last position).  Tokens are checked on the host.
+template <int D>
+__global__ void __launch_bounds__(256)
+embed_ln_rows_kernel(const long long* __restrict__ tokens, int T, const float* __restrict__ words,
+                     const float* __restrict__ positions, const float* __restrict__ gamma, const float* __restrict__ beta,
+                     float* __restrict__ out_f32, __nv_bfloat16* __restrict__ out_bf16, int rows, int vocab, int split3,
+                     int* __restrict__ targets) {
+  constexpr int NV = D / 128;
+  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  const int lane = threadIdx.x & 31;
+  const int pos = row % T;
+  long long tok = tokens[row];
+  tok = tok < 0 ? 0 : (tok >= vocab ? vocab - 1 : tok);
+  if (lane == 0) targets[row] = pos + 1 < T ? static_cast<int>(tokens[row + 1]) : -1;
+  const float4* wp = reinterpret_cast<const float4*>(words + tok * D);
+  const float4* pp = reinterpret_cast<const float4*>(positions + static_cast<long long>(pos) * D);
+  float4 v[NV];
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const float4 a = __ldg(wp + i * 32 + lane);
+    const float4 b = __ldg(pp + i * 32 + lane);
+    v[i] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+    s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
+  }
+  const float mean = warp_sum(s) * (1.0f / D);
+  float ss = 0.f;
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
+    ss += (a * a + b * b) + (c * c + d * d);
+  }
+  const float rstd = rsqrtf(warp_sum(ss) * (1.0f / D) + 1e-8f);
+#pragma unroll
+  for (int i = 0; i < NV; ++i) {
+    const float4 g = __ldg(reinterpret_cast<const float4*>(gamma) + i * 32 + lane);
+    const float4 b = __ldg(reinterpret_cast<const float4*>(beta) + i * 32 + lane);
+    float4 o = make_float4((v[i].x - mean) * rstd * g.x + b.x, (v[i].y - mean) * rstd * g.y + b.y,
+                           (v[i].z - mean) * rstd * g.z + b.z, (v[i].w - mean) * rstd * g.w + b.w);
+    reinterpret_cast<float4*>(out_f32 + static_cast<long long>(row) * D)[i * 32 + lane] = o;
+    if (split3) {
+      uint2 hi, lo;
+      pack_split2(o.x, o.y, hi.x, lo.x);
+      pack_split2(o.z, o.w, hi.y, lo.y);
+      uint2* dst = reinterpret_cast<uint2*>(out_bf16 + static_cast<long long>(row) * 3 * D) + i * 32 + lane;
+      dst[0] = hi; dst[D / 4] = lo; dst[D / 2] = hi;
+    } else {
+      uint2 pk;
+      pk.x = pack_bf16(o.x, o.y);
+      pk.y = pack_bf16(o.z, o.w);
+      reinterpret_cast<uint2*>(out_bf16 + static_cast<long long>(row) * D)[i * 32 + lane] = pk;
+    }
+  }
+}
+
+// One warp per text row: folds the row's n_parts LM-head partials (gemm.cuh EPI_LSE) into lse, the target's log-probability
+// and the label-smoothed loss of SmoothLabelCrossEntropyLoss (reference layers/decoder.py:620-671, eps 0.1): with q the
+// smoothed one-hot and lp = x - lse,
+//   sum_c q_c (log q_c - lp_c) = sum q log q - (1 - eps) lp_t - eps / (V - 1) (sum_c lp_c - lp_t),  sum_c lp_c = sum x - V lse.
+// Lane l folds parts l, l + 32, .. in order, then the lanes merge in a fixed tree: reproducible, no atomics.
+// Row n * T + t scores token t + 1 of caption n (t < T - 1): logprob_out[n * (T - 1) + t]; it counts towards the loss when
+// need_predict[n, t + 1] == 1 and the token is not the padding id 0 (:940-960, :640-643).
+__global__ void __launch_bounds__(256)
+lse_combine_kernel(const float4* __restrict__ parts, int n_parts, int rows, int T, int V, const int* __restrict__ targets,
+                   const long long* __restrict__ need_predict, float eps, float* __restrict__ logprob_out,
+                   float* __restrict__ row_loss, int* __restrict__ row_valid) {
+  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  const int lane = threadIdx.x & 31;
+  float m = -INFINITY, se = 0.f, xt = 0.f;
+  double sx = 0.0;
+  for (int k = lane; k < n_parts; k += 32) {
+    const float4 q = __ldg(parts + static_cast<long long>(row) * n_parts + k);
+    if (q.x != -INFINITY) {
+      const float nm = fmaxf(m, q.x);
+      se = ((m == -INFINITY) ? 0.f : se * expf(m - nm)) + q.y * expf(q.x - nm);
+      m = nm;
+    }
+    sx += static_cast<double>(q.z);
+    xt += q.w;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float m_o = __shfl_xor_sync(0xffffffffu, m, o);
+    const float s_o = __shfl_xor_sync(0xffffffffu, se, o);
+    const float nm = fmaxf(m, m_o);
+    se = ((m == -INFINITY) ? 0.f : se * expf(m - nm)) + ((m_o == -INFINITY) ? 0.f : s_o * expf(m_o - nm));
+    m = nm;
+    sx += __shfl_xor_sync(0xffffffffu, sx, o);
+    xt += __shfl_xor_sync(0xffffffffu, xt, o);
+  }
+  if (lane != 0) return;
+  const int t = row % T;
+  const int n = row / T;
+  const int tgt = targets[row];
+  float loss = 0.f;
+  int valid = 0;
+  if (t + 1 < T) {
+    const double lse = static_cast<double>(m) + log(static_cast<double>(se));
+    const double lp = static_cast<double>(xt) - lse;
+    logprob_out[static_cast<long long>(n) * (T - 1) + t] = static_cast<float>(lp);
+    valid = (need_predict[row + 1] == 1 && tgt != 0) ? 1 : 0;
+    if (valid) {
+      const double e = eps, off = e / (V - 1);
+      const double qlogq = (1.0 - e) * log(1.0 - e) + e * log(off);
+      const double sum_lp = sx - static_cast<double>(V) * lse;
+      loss = static_cast<float>(qlogq - (1.0 - e) * lp - off * (sum_lp - lp));
+    }
+  }
+  row_loss[row] = loss;
+  row_valid[row] = valid;
+}
+
+// Mean of the valid rows' losses (NaN when there are none): one CTA, fixed-order tree over strided partial sums.
+__global__ void __launch_bounds__(1024) loss_mean_kernel(const float* __restrict__ row_loss, const int* __restrict__ row_valid,
+                                                         int rows, float* __restrict__ out) {
+  __shared__ double s_sum[1024];
+  __shared__ int s_cnt[1024];
+  double a = 0.0;
+  int c = 0;
+  for (int r = threadIdx.x; r < rows; r += blockDim.x) {
+    a += row_loss[r];
+    c += row_valid[r];
+  }
+  s_sum[threadIdx.x] = a;
+  s_cnt[threadIdx.x] = c;
+  __syncthreads();
+  for (int w = blockDim.x / 2; w > 0; w >>= 1) {
+    if (static_cast<int>(threadIdx.x) < w) {
+      s_sum[threadIdx.x] += s_sum[threadIdx.x + w];
+      s_cnt[threadIdx.x] += s_cnt[threadIdx.x + w];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) out[0] = s_cnt[0] > 0 ? static_cast<float>(s_sum[0] / s_cnt[0]) : __int_as_float(0x7fc00000);
+}
+
+// ------------------------------------------------------------------------------------------------
 // Greedy selection = the body of AutoRegressiveBeamSearch.search for beam 1 / per-node 1
 // (reference layers/decoder.py:258-273 first step, :313-417 loop): no-repeat scatter(-10000) on the
 // input token (not on the first step), EOS forcing, log_softmax, argmax (lowest index on exact ties),

@@ -601,6 +601,96 @@ class GitB200CaptioningModel(nn.Module):
         sl['pending'] = pend
         return pend
 
+    # ---------------------------------------------------------------- caption scoring
+    def _score_args(self, batch):
+        """Host-side checks of a score() batch (before any engine is touched) -> (image, B, tokens, need_predict, image_index),
+        the last three as CPU tensors."""
+        for key in ('context', 'bi_valid_mask_caption'):
+            if key in batch:
+                raise NotImplementedError("score(): %r batches are not supported" % key)
+        for key in ('image', 'caption_tokens', 'need_predict'):
+            if key not in batch:
+                raise ValueError("score(): batch needs %r" % key)
+        image = batch['image']
+        if self._is_ragged(image):
+            B = len(image)
+        elif isinstance(image, (list, tuple)):
+            if not image or image[0].dim() != 4:
+                raise ValueError('score(): video frames must be a list of [B, 3, H, W] tensors')
+            B = int(image[0].shape[0])
+        else:
+            if image.dim() != 4:
+                raise ValueError("score(): 'image' must be [B, 3, H, W] (got %s)" % (tuple(image.shape),))
+            B = int(image.shape[0])
+        tokens = torch.as_tensor(batch['caption_tokens']).detach().cpu()
+        need = torch.as_tensor(batch['need_predict']).detach().cpu()
+        if tokens.dim() != 2 or tokens.dtype.is_floating_point:
+            raise ValueError("score(): 'caption_tokens' must be an integer [N, T] tensor")
+        N, T = tokens.shape
+        if not 2 <= T <= MAX_POS:
+            raise ValueError('score(): T = %d positions; 2 <= T <= %d' % (T, MAX_POS))
+        if N < 1:
+            raise ValueError('score(): no captions')
+        if tuple(need.shape) != (N, T):
+            raise ValueError("score(): 'need_predict' is %s, 'caption_tokens' %s" % (tuple(need.shape), (N, T)))
+        if bool(((need != 0) & (need != 1)).any()):
+            raise ValueError("score(): 'need_predict' must hold 0 / 1")
+        if int(tokens.min()) < 0 or int(tokens.max()) >= VOCAB:
+            raise ValueError('score(): token ids must lie in [0, %d)' % VOCAB)
+        index = batch.get('image_index')
+        if index is not None:
+            index = torch.as_tensor(index).detach().cpu()
+            if tuple(index.shape) != (N,) or index.dtype.is_floating_point:
+                raise ValueError("score(): 'image_index' must be an integer [N] tensor")
+            if int(index.min()) < 0 or int(index.max()) >= B:
+                raise ValueError("score(): 'image_index' must lie in [0, %d)" % B)
+        elif N != B:
+            raise ValueError("score(): %d captions for %d images need an 'image_index'" % (N, B))
+        if not bool(((need[:, 1:] == 1) & (tokens[:, 1:] != 0)).any()):
+            raise ValueError('score(): no position to predict (need_predict == 1 with a non-zero target)')
+        return image, B, tokens.long(), need.long(), index
+
+    @torch.no_grad()
+    def score(self, batch):
+        """Teacher-forced scoring of given captions in one pass (the reference's training-branch forward,
+        layers/decoder.py:916-972, with dropout off).
+
+        batch: {'image': as for `model(batch)` (tensor, list of frames, or ragged list of [3, H_b, W_b] images),
+                'caption_tokens': LongTensor[N, T] (CLS .. SEP, 0-padded), 'need_predict': [N, T] of 0 / 1,
+                'image_index'?: LongTensor[N] = the image of each caption (default: caption n, image n)}.
+        Returns {'token_logprobs': fp32 [N, T-1] = log_softmax(logits[n, t])[caption_tokens[n, t+1]],
+                 'vl_l_loss': fp32 scalar = the reference's SmoothLabelCrossEntropyLoss (eps 0.1) over the positions with
+                 need_predict[n, t+1] == 1 and a non-zero target}.
+        Captions of one image share its encoder pass.  The arguments are checked on the host (token ids, shapes, indices)."""
+        image, B, tokens, need, index = self._score_args(batch)
+        N, T = tokens.shape
+        ragged = self._is_ragged(image)
+        lib, _ = self._ensure_engine(0)
+        sl = self._slots[0]
+        if sl['pending'] is not None:
+            sl['pending'].result()
+        eng = sl['engine']
+        dev = self._device()
+        if ragged:
+            x, B, sizes = self._pack_ragged(image)
+            frames = 0
+        else:
+            x, B, frames = self._pack_images(image)
+        tok_d = tokens.to(dev).contiguous()
+        need_d = need.to(dev).contiguous()
+        idx_d = index.to(device=dev, dtype=torch.int32).contiguous() if index is not None else None
+        lp = torch.empty((N, T - 1), dtype=torch.float32, device=dev)
+        loss = torch.empty((1,), dtype=torch.float32, device=dev)
+        if ragged:
+            _lib.check(lib.gitb200_set_image_sizes(eng, *self._sizes_arg(sizes)), eng, 'set_image_sizes')
+        else:
+            _lib.check(lib.gitb200_set_input_size(eng, int(x.shape[-2]), int(x.shape[-1])), eng, 'set_input_size')
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        _lib.check(lib.gitb200_score(eng, x.data_ptr(), B, frames, tok_d.data_ptr(), need_d.data_ptr(),
+                                     idx_d.data_ptr() if idx_d is not None else None, N, T, lp.data_ptr(), loss.data_ptr(),
+                                     stream), eng, 'score')
+        return {'token_logprobs': lp, 'vl_l_loss': loss[0]}
+
     def _sampling_setup(self, search_param, sp, B, dev):
         """search_param of the reference's decoder.search (layers/decoder.py:224-232) -> the uniforms the engine draws with."""
         if not search_param:

@@ -62,7 +62,7 @@ enum { GITB200_F32 = 0, GITB200_BF16 = 1, GITB200_I64 = 2 };
 int gitb200_create(const gitb200_config* cfg, int device, gitb200_engine** out);
 void gitb200_destroy(gitb200_engine* h);
 const char* gitb200_last_error(const gitb200_engine* h);
-/* ABI version of the library (bumped on any signature change): 8 (gitb200_op_attention_ex, gitb200_op_decode_attention). */
+/* ABI version of the library (bumped on any signature change): 9 (gitb200_score, gitb200_op_text_attention). */
 int gitb200_abi_version(void);
 
 /* Replaces: torch_common.load_state_dict -> module parameters           torch_common.py:93-145.
@@ -152,6 +152,21 @@ int gitb200_generate_host_async(gitb200_engine* h, const float* images_host, int
                                 int64_t* tokens_out_host, float* logprobs_out_host, void* stream);
 int gitb200_generate_finish(gitb200_engine* h, int32_t* out_len_host);
 
+/* Replaces: the training branch of CaptioningModel.forward_one_ce with dropout off  layers/decoder.py:916-972, i.e.
+ * TransformerDecoderTextualHead.forward over given captions :521-600 and SmoothLabelCrossEntropyLoss :620-671 (eps 0.1,
+ * padding id 0 ignored).  Scores N captions of T positions against the images in ONE teacher-forced pass.
+ * images_dev, batch, frames as gitb200_generate (gitb200_set_input_size, and gitb200_set_image_sizes for the next call,
+ * apply).  tokens_dev int64 [N, T]: CLS .. SEP rows padded with 0, ids in [0, vocab) (not checked here; out-of-range ids
+ * are clamped).  need_predict_dev int64 [N, T] of 0 / 1 (the data layout of train.py:38-61).  image_index_dev int32 [N] in
+ * [0, batch): the image of each caption, or NULL when N == batch (caption n, image n); captions of one image share its
+ * encoder pass and image K/V.  2 <= T <= max_positions.
+ * token_logprob_out_dev fp32 [N, T - 1]: log_softmax(logits[n, t])[tokens[n, t + 1]] for every t.
+ * loss_out_dev fp32 [1] or NULL: the mean smoothed loss over the positions with need_predict[n, t + 1] == 1 and
+ * tokens[n, t + 1] != 0 (NaN when there are none; the reference asserts).  Enqueued on `stream` without a host sync. */
+int gitb200_score(gitb200_engine* h, const float* images_dev, int batch, int frames, const int64_t* tokens_dev,
+                  const int64_t* need_predict_dev, const int32_t* image_index_dev, int n_captions, int positions,
+                  float* token_logprob_out_dev, float* loss_out_dev, void* stream);
+
 /* Measurement hook (bench.py's roofline): device time, by CUDA events on the engine's stream, of the decode loop of the
  * last generate on this engine -- first step launch to last -- with the number of step launches in it and whether each
  * was the single decode_mega_kernel launch.  Waits for that loop to finish.  No reference counterpart. */
@@ -231,6 +246,16 @@ int gitb200_op_decode_attention(const float* qkv_dev, int n_partials, const floa
                                 const void* img_v_dev, void* txt_k_dev, void* txt_v_dev, const int32_t* src_row_dev,
                                 void* ctx_dev, int B, int beam, int M, const int32_t* img_lens_host, int T_alloc, int pos,
                                 int D, int fp32, int grid, void* stream);
+
+/* Caption scoring's attention (text_attn_wgmma_kernel, or text_attn_f32_kernel when fp32 != 0): text row t of caption n
+ * attends to the image keys of image image_index[n] and to text keys 0 .. t of caption n; softmax(q k^T / 8) v per head.
+ * q / txt_k / txt_v [N * T, H * 64] rows (caption n at rows n * T ..), img_k / img_v [B * M, H * 64] (image b at rows b * M ..):
+ * bf16, or fp32 when fp32 != 0.  img_lens_host: NULL (every image has M keys) or B key counts in 1..M.  image_index_host:
+ * NULL (N == B, caption n uses image n) or N indices in 0..B-1.  out_dev bf16 [N * T, H * 64], or split rows
+ * [N * T, 3 * H * 64] ([hi | lo | hi]) when fp32 != 0. */
+int gitb200_op_text_attention(const void* q_dev, const void* txt_k_dev, const void* txt_v_dev, const void* img_k_dev,
+                              const void* img_v_dev, void* out_dev, int N, int T, int B, int M, const int32_t* img_lens_host,
+                              const int32_t* image_index_host, int H, int fp32, void* stream);
 
 /* ---- test-time image transform on the GPU ----------------------------------------------------------------
  * Replaces: get_image_transform(param)(pil_image)                                       inference.py:111-132
