@@ -238,10 +238,14 @@ struct MegaAFrag {
   uint32_t lo[6][8];   // row g     : 16 contiguous k per entry (four k-steps)
   uint32_t hi[6][8];   // row g + 8
 };
-// 32 contiguous bytes, L1-bypassing (sm_90 has no 256-bit loads: two 128-bit ones)
-__device__ __forceinline__ void ldcg_256(uint32_t (&r)[8], const void* p) {
-  asm volatile("ld.global.cg.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "l"(p));
-  asm volatile("ld.global.cg.v4.u32 {%0, %1, %2, %3}, [%4];"
+// 32 contiguous bytes (sm_90 has no 256-bit loads: two 128-bit ones).  Cached in L1: each of the two instructions covers
+// half of every 32-byte sector of the four lanes' 128-byte line, so with L2-only (.cg) loads the second one fetched the
+// same sectors from L2 again -- twice the operand's bytes through the SM's L2 port per phase.  Weak loads are safe here:
+// the operand was written before the grid barrier this CTA passed, whose acquire load invalidates the SM's L1
+// (CCTL.IVALL), or by an earlier launch.
+__device__ __forceinline__ void ld_256(uint32_t (&r)[8], const void* p) {
+  asm volatile("ld.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "l"(p));
+  asm volatile("ld.global.v4.u32 {%0, %1, %2, %3}, [%4];"
                : "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
                : "l"(static_cast<const uint8_t*>(p) + 16));
 }
@@ -252,12 +256,12 @@ __device__ __forceinline__ void mega_load_a(MegaAFrag& a, const __nv_bfloat16* A
   const __nv_bfloat16* p1 = A + static_cast<long long>(r1) * lda + kh * 384 + 16 * t;
 #pragma unroll
   for (int j = 0; j < 6; ++j) {
-    if (r0 < rows) ldcg_256(a.lo[j], p0 + 64 * j);
+    if (r0 < rows) ld_256(a.lo[j], p0 + 64 * j);
     else {
 #pragma unroll
       for (int e = 0; e < 8; ++e) a.lo[j][e] = 0u;
     }
-    if (r1 < rows) ldcg_256(a.hi[j], p1 + 64 * j);
+    if (r1 < rows) ld_256(a.hi[j], p1 + 64 * j);
     else {
 #pragma unroll
       for (int e = 0; e < 8; ++e) a.hi[j][e] = 0u;
