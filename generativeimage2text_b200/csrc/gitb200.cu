@@ -152,6 +152,7 @@ struct gitb200_engine {
   DevBuf x, h, qkv, ctx, u, feats, feats_f32, pos_interp;   // encoder
   DevBuf pt, pxd, phd, pq, pctx, pu;                        // prefill
   DevBuf img_kv, txt_kv, src_row[2];                        // caches
+  size_t txt_kv_eb = 0;                                     // element size (kvb()) the text cache was last zeroed for
   DevBuf xd_t, hd_t, qkv_t, ctx_t, t_t, u_t, logits;        // decode step
   DevBuf y_t, qb_t, mega_bar;                               // decode_mega_kernel: pre-LN sums, bf16 q, grid-barrier counters
   DevBuf state, next_token, logprob_sum, tokens_i64, stage_img, stage_tok, stage_lp, prefix_dev;
@@ -1247,10 +1248,12 @@ static int prefill_impl(gitb200_engine* h, int B, int beam, int T_alloc, float* 
   {
     // decode_mega_kernel fetches whole 64-position boxes of the text cache and masks the positions past the caption's end
     // by giving them probability 0 -- which only works if what lies there is finite: a fresh allocation is zeroed once
-    // (afterwards the buffer only ever holds K/V values or zeros)
+    // (afterwards the buffer only ever holds K/V values or zeros of one element size).  A parity switch keeps the buffer
+    // but changes the element size: fp32 K/V read as bf16 pairs hold Inf / NaN patterns, so the cache is zeroed again.
     const void* before = h->txt_kv.p;
     CK(h->txt_kv.ensure(static_cast<long long>(nl) * 2 * R * T_alloc * D * kvb));
-    if (h->txt_kv.p != before) CK(cudaMemsetAsync(h->txt_kv.p, 0, h->txt_kv.cap, st));
+    if (h->txt_kv.p != before || h->txt_kv_eb != h->kvb()) CK(cudaMemsetAsync(h->txt_kv.p, 0, h->txt_kv.cap, st));
+    h->txt_kv_eb = h->kvb();
   }
   CK(h->src_row[0].ensure(static_cast<size_t>(R) * T_alloc * 4));
   CK(h->src_row[1].ensure(static_cast<size_t>(R) * T_alloc * 4));

@@ -292,7 +292,9 @@ int gitb200_preproc_run(gitb200_preproc* p, const uint8_t* src, int64_t src_byte
 int gitb200_preproc_coeffs(int in_size, int out_size, int32_t* ksize_out, int32_t* bounds_out, int32_t* kk_out, int kk_cap);
 
 /* Debug: copies one decode-step work buffer of the engine ("x", "y" fp32 [rows,768]; "hb", "ctx", "qb" bf16 [rows,768];
- * "ub" bf16 [rows,3072]) to host memory after a device synchronise.  Returns bytes copied or -1. */
+ * "ub" bf16 [rows,3072]) or cache ("img_kv": the image K/V [layer][k|v][image][token][768] of the last prefill, batch x
+ * tokens rows; "txt_kv": the text K/V [layer][k|v][row][T_alloc][768], T_alloc = bytes / (layers * 2 * rows * 768 * element
+ * size); both bf16, fp32 in parity mode) to host memory after a device synchronise.  Returns bytes copied or -1. */
 long long gitb200_debug_read(gitb200_engine* h, const char* name, void* out_host, long long max_bytes);
 /* Debug aid: in-situ timeline of the decode-step kernels. enable != 0 arms it; enable == 0 copies up to
  * max_entries (globaltimer ns, kernel id) pairs to out_host, disarms, and returns the number of entries. */
