@@ -11,9 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libgitb200.so')
 SOURCES = ['gitb200.cu']
-DEPS = ['gitb200.cu', 'engine_api.inc', 'ptx.cuh', 'gemm.cuh', 'rowops.cuh', 'attention.cuh', 'decode_mega.cuh',
-        'search.cuh', 'preproc.cuh', 'preproc_api.inc',
-        os.path.join('..', '..', 'include', 'gitb200.h')]
+HEADER = os.path.join(HERE, '..', 'include', 'gitb200.h')
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC', '-shared']
 
@@ -25,11 +23,16 @@ def _nvcc():
     raise RuntimeError('nvcc not found: libgitb200.so cannot be built (there is no CPU implementation)')
 
 
+def deps():
+    """Every file the library is compiled from: all of csrc/ (sources and the headers they include) and the C header."""
+    return [os.path.join(CSRC, f) for f in sorted(os.listdir(CSRC))] + [HEADER]
+
+
 def is_stale():
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    return any(os.path.getmtime(os.path.join(CSRC, d)) > t for d in DEPS)
+    return any(os.path.getmtime(d) > t for d in deps())
 
 
 def build(force=False, verbose=False):

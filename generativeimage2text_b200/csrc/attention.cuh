@@ -3,14 +3,17 @@
 // flash_attn_wgmma_kernel : non-causal softmax(q k^T / 8) v over S keys for every (batch, head); used by the
 //   ViT blocks (reference layers/CLIP/model.py:189-197 -> nn.MultiheadAttention -> SDPA, no mask) and by
 //   the one-off image-row pass of the decoder (image rows attend image rows only, reference
-//   layers/decoder.py:119-120; layers/bert/modeling_bert.py:41-47,138-152).  TMA-fed K/V blocks on an mbarrier
-//   ring, S = Q K^T and O = P V as wgmma, online softmax in registers.
-// flash_attn_kernel : the same with cp.async loads and warp-level mma.sync, for batches that are not stored back to back.
+//   layers/decoder.py:119-120; layers/bert/modeling_bert.py:41-47,138-152).  Batches are stored back to back.
+// text_attn_wgmma_kernel : the text rows of a caption batch in one pass (caption scoring).  Both run attn_wg_tile:
+//   TMA-fed K/V blocks on an mbarrier ring, S = Q K^T and O = P V as wgmma, online softmax in registers.
 //
 // decode_attn_kernel : one new text row per sequence against [image K/V || text K/V] (the KV-cached form of
 //   reference layers/decoder.py:121-123 + modeling_bert.py:124-152).  Pure HBM streaming: every K/V row is
 //   read once with 128-bit loads; image K/V are shared by the beams of an image; the new token's K/V are
 //   appended to the text cache by the same kernel.
+//
+// attn_f32_kernel, text_attn_f32_kernel, decode_attn_f32_kernel : the three in plain fp32 for parity mode, one warp per
+//   query row (attn_row_f32).
 #pragma once
 #include "ptx.cuh"
 #include "rowops.cuh"
@@ -23,227 +26,59 @@ struct AttnParams {
   const __nv_bfloat16* v;
   __nv_bfloat16* out;
   int B, S, H;
-  long long q_rs, kv_rs, q_bs, kv_bs, o_rs, o_bs;  // row / batch strides in elements
+  long long q_rs, kv_rs, q_bs, kv_bs, o_rs, o_bs;  // row / batch strides in elements (batches back to back: q_bs = S q_rs)
   float scale_log2;                                 // (1/sqrt(64)) * log2(e)
   const int* seq_lens;                              // flash_attn_wgmma_kernel<true>: [B] valid rows of each batch (<= S)
 };
 
-__device__ __forceinline__ void attn_load_tile(uint32_t smem_base, const __nv_bfloat16* g, long long row_stride,
-                                               int row0, int nrows, int S, int tid, int nthreads) {
-  for (int idx = tid; idx < nrows * 8; idx += nthreads) {
-    const int r = idx >> 3;
-    const int c = idx & 7;
-    const bool valid = (row0 + r) < S;
-    const int gr = valid ? (row0 + r) : (S - 1);
-    const __nv_bfloat16* src = g + static_cast<long long>(gr) * row_stride + c * 8;
-    cp_async_16(smem_base + r * 128 + ((c ^ (r & 7)) << 4), src, valid);
-  }
-}
-
-template <int NW>
-__global__ void __launch_bounds__(NW * 32) flash_attn_kernel(const AttnParams p) {
-  constexpr int QROWS = NW * 16;
-  constexpr int KC = 64;
-  __shared__ __align__(128) uint8_t sQ[QROWS * 128];
-  __shared__ __align__(128) uint8_t sK[2][KC * 128];
-  __shared__ __align__(128) uint8_t sV[2][KC * 128];
-
-  const int tid = threadIdx.x;
-  const int warp = tid >> 5;
-  const int lane = tid & 31;
-  const int q_row0 = blockIdx.x * QROWS;
-  const int h = blockIdx.y;
-  const int b = blockIdx.z;
-  const __nv_bfloat16* qg = p.q + b * p.q_bs + h * 64;
-  const __nv_bfloat16* kg = p.k + b * p.kv_bs + h * 64;
-  const __nv_bfloat16* vg = p.v + b * p.kv_bs + h * 64;
-  const int nchunks = (p.S + KC - 1) / KC;
-
-  attn_load_tile(smem_u32(sQ), qg, p.q_rs, q_row0, QROWS, p.S, tid, NW * 32);
-  attn_load_tile(smem_u32(sK[0]), kg, p.kv_rs, 0, KC, p.S, tid, NW * 32);
-  attn_load_tile(smem_u32(sV[0]), vg, p.kv_rs, 0, KC, p.S, tid, NW * 32);
-  cp_async_commit();
-
-  uint32_t qa[4][4];
-  float o[8][4];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
-  }
-  float m_run[2] = {-INFINITY, -INFINITY};
-  float l_run[2] = {0.f, 0.f};
-
-  for (int c = 0; c < nchunks; ++c) {
-    const int buf = c & 1;
-    if (c + 1 < nchunks) {
-      attn_load_tile(smem_u32(sK[buf ^ 1]), kg, p.kv_rs, (c + 1) * KC, KC, p.S, tid, NW * 32);
-      attn_load_tile(smem_u32(sV[buf ^ 1]), vg, p.kv_rs, (c + 1) * KC, KC, p.S, tid, NW * 32);
-      cp_async_commit();
-      cp_async_wait<1>();
-    } else {
-      cp_async_wait<0>();
-    }
-    __syncthreads();
-    if (c == 0) {
-      const int row = warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {
-        const int chunk = 2 * kk + (lane >> 4);
-        ldmatrix_x4(qa[kk][0], qa[kk][1], qa[kk][2], qa[kk][3], smem_u32(sQ) + row * 128 + ((chunk ^ (row & 7)) << 4));
-      }
-    }
-    // ---- S = Q K^T for this chunk -------------------------------------------------------------
-    float s[8][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
-      const int krow = 8 * j + (lane & 7);
-#pragma unroll
-      for (int kk2 = 0; kk2 < 2; ++kk2) {
-        const int chunk = 4 * kk2 + (lane >> 3);
-        uint32_t b0, b1, b2, b3;
-        ldmatrix_x4(b0, b1, b2, b3, smem_u32(sK[buf]) + krow * 128 + ((chunk ^ (krow & 7)) << 4));
-        mma_bf16_16816(s[j], qa[2 * kk2], b0, b1);
-        mma_bf16_16816(s[j], qa[2 * kk2 + 1], b2, b3);
-      }
-    }
-    // ---- mask the tail, online softmax ---------------------------------------------------------
-    const int key0 = c * KC + 2 * (lane & 3);
-    float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int key = key0 + 8 * j;
-      if (key >= p.S) { s[j][0] = -INFINITY; s[j][2] = -INFINITY; }
-      if (key + 1 >= p.S) { s[j][1] = -INFINITY; s[j][3] = -INFINITY; }
-      mx[0] = fmaxf(mx[0], fmaxf(s[j][0], s[j][1]));
-      mx[1] = fmaxf(mx[1], fmaxf(s[j][2], s[j][3]));
-    }
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
-      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
-    }
-    float corr[2], m_new[2];
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      m_new[i] = fmaxf(m_run[i], mx[i]);
-      corr[i] = exp2f((m_run[i] - m_new[i]) * p.scale_log2);
-      m_run[i] = m_new[i];
-      l_run[i] *= corr[i];
-    }
-    uint32_t pa[4][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float p0 = exp2f((s[j][0] - m_new[0]) * p.scale_log2);
-      const float p1 = exp2f((s[j][1] - m_new[0]) * p.scale_log2);
-      const float p2 = exp2f((s[j][2] - m_new[1]) * p.scale_log2);
-      const float p3 = exp2f((s[j][3] - m_new[1]) * p.scale_log2);
-      l_run[0] += p0 + p1;
-      l_run[1] += p2 + p3;
-      pa[j >> 1][(j & 1) * 2 + 0] = pack_bf16(p0, p1);
-      pa[j >> 1][(j & 1) * 2 + 1] = pack_bf16(p2, p3);
-      o[j][0] *= corr[0];
-      o[j][1] *= corr[0];
-      o[j][2] *= corr[1];
-      o[j][3] *= corr[1];
-    }
-    // ---- O += P V -------------------------------------------------------------------------------
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      const int vrow = 16 * kk + ((lane >> 3) & 1) * 8 + (lane & 7);
-#pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        const int chunk = 2 * jj + (lane >> 4);
-        uint32_t b0, b1, b2, b3;
-        ldmatrix_x4_trans(b0, b1, b2, b3, smem_u32(sV[buf]) + vrow * 128 + ((chunk ^ (vrow & 7)) << 4));
-        mma_bf16_16816(o[2 * jj], pa[kk], b0, b1);
-        mma_bf16_16816(o[2 * jj + 1], pa[kk], b2, b3);
-      }
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    l_run[i] += __shfl_xor_sync(0xffffffffu, l_run[i], 1);
-    l_run[i] += __shfl_xor_sync(0xffffffffu, l_run[i], 2);
-  }
-  const float inv0 = 1.0f / l_run[0];
-  const float inv1 = 1.0f / l_run[1];
-  const int r0 = q_row0 + warp * 16 + (lane >> 2);
-  const int r1 = r0 + 8;
-  __nv_bfloat16* og = p.out + b * p.o_bs + h * 64 + 2 * (lane & 3);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    if (r0 < p.S)
-      *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r0) * p.o_rs + 8 * j) = pack_bf16(o[j][0] * inv0, o[j][1] * inv0);
-    if (r1 < p.S)
-      *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r1) * p.o_rs + 8 * j) = pack_bf16(o[j][2] * inv1, o[j][3] * inv1);
-  }
-}
-
 // ------------------------------------------------------------------------------------------------
-// flash_attn_wgmma_kernel: the same non-causal attention on Hopper's warpgroup tensor cores, for any S (ViT blocks with
-// 197 / 257 keys, the image-row prefill, 6-frame video with 1182 keys, 30 x 40 VQA grids with 1201).
-//   One CTA = one warpgroup per (64 query rows, head, batch).  Thread 0 loads the Q tile and 64-key K / V blocks by TMA
-//   (128B-swizzled 64 x 64 bf16 boxes) into a two-stage ring, each stage completing on its own mbarrier, so block i + 1
-//   is in flight while block i is computed.  Per block: S = Q K^T as four wgmma m64n64k16 with both operands in shared
-//   memory; online softmax in registers (thread = two query rows, a quad of lanes shares a row); O += P V as four wgmma
-//   with P straight from registers (the accumulator layout of S is the A-fragment layout) and V as an MN-major B operand
-//   (V stays [key][dim] as TMA delivered it).  The row sum adds the bf16-rounded weights that P V multiplies, so the
-//   output is their exact weighted mean.  With the fp32 weights summed instead (measured with the mma.sync kernel on an
-//   H100), the engine's logit error on the decisive-margin golden of tests/test_gpu_parity.py was 0.0625 instead of
-//   0.0556, below that test's required factor 4 under the golden's smallest decision margin (0.247).
+// attn_wg_tile: softmax(Q K^T / 8) V for one 64-row query tile of one head on Hopper's warpgroup tensor cores, the block
+// loop of flash_attn_wgmma_kernel and text_attn_wgmma_kernel.
+//   One CTA = one warpgroup.  Thread 0 loads the Q tile and 64-key K / V blocks by TMA (128B-swizzled 64 x 64 bf16 boxes)
+//   into a two-stage ring, each stage completing on its own mbarrier, so block i + 1 is in flight while block i is
+//   computed.  Per block: S = Q K^T as four wgmma m64n64k16 with both operands in shared memory; online softmax in
+//   registers (thread = two query rows, a quad of lanes shares a row); O += P V as four wgmma with P straight from
+//   registers (the accumulator layout of S is the A-fragment layout) and V as an MN-major B operand (V stays [key][dim] as
+//   TMA delivered it).  The row sum adds the bf16-rounded weights that P V multiplies, so the output is their exact
+//   weighted mean.  With the fp32 weights summed instead (measured with an mma.sync kernel on an H100), the engine's logit
+//   error on the decisive-margin golden of tests/test_gpu_parity.py was 0.0625 instead of 0.0556, below that test's
+//   required factor 4 under the golden's smallest decision margin (0.247).
+//
+// The caller chooses the keys through two callables:
+//   load_kv(blk, sK, sV, bar)  thread 0: issue K / V block blk by TMA into sK / sV (8192 B each), completing on bar;
+//   mask(blk, s)               set the scores of block blk that a row must not see to -inf.  Every row has to keep at
+//                              least one key of every block (the running max stays finite).
+// Thread 0 prefetches the tensor map descriptors before the call.  On return o holds this thread's outputs, normalised:
+// register 4j + e is row warp * 16 + lane / 4 (+ 8 for e >= 2) of the tile, dims 8j + 2 (lane % 4) + (e & 1).
 // ------------------------------------------------------------------------------------------------
 constexpr int kAttnWgRows = 64;                 // query rows per CTA = keys per K / V block
 constexpr int kAttnWgSmem = 5 * 8192 + 64 + 1024;   // Q | K x 2 | V x 2 | barriers | alignment slack
 
-// kRagged (ragged image batches): batch b occupies a slot of p.S rows of which the first p.seq_lens[b] are valid; the
-// batch is computed exactly as a uniform call with S = seq_lens[b] would compute it (the key blocks and query tiles past
-// its length are skipped, not masked) and its output rows past that length are written as zeros.
-template <bool kRagged>
-__global__ void __launch_bounds__(128) flash_attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ,
-                                                              const __grid_constant__ CUtensorMap tmK,
-                                                              const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
+template <class LoadKV, class Mask>
+__device__ __forceinline__ void attn_wg_tile(const CUtensorMap* tmQ, int q_col, int q_row, int nblk, float scale_log2,
+                                             const LoadKV& load_kv, const Mask& mask, float (&o)[32]) {
   extern __shared__ __align__(1024) uint8_t attn_smem_raw[];
   uint8_t* smem = attn_smem_raw + ((1024u - (smem_u32(attn_smem_raw) & 1023u)) & 1023u);
   uint8_t* sQ = smem;
   uint8_t* sK = smem + 8192;                     // [2 stages][64 keys][128 B]
   uint8_t* sV = smem + 3 * 8192;
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 5 * 8192);   // [0] Q, [1 + stage] K | V
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int h = blockIdx.y, b = blockIdx.z;
-  const int S = kRagged ? p.seq_lens[b] : p.S;
-  const int q0 = blockIdx.x * kAttnWgRows;
-  const int row_base = b * p.S;                  // rows of batch b in the [B * S, H * 64] q / k / v views
-  const int nblk = (S + kAttnWgRows - 1) / kAttnWgRows;
-  if (kRagged && q0 >= S) {                      // a query tile of the padding: zeros, no arithmetic
-    __nv_bfloat16* og = p.out + b * p.o_bs + h * 64;
-    for (int i = tid; i < kAttnWgRows * 8; i += 128) {
-      const int r = q0 + (i >> 3);
-      if (r < p.S) *reinterpret_cast<uint4*>(og + static_cast<long long>(r) * p.o_rs + (i & 7) * 8) = make_uint4(0, 0, 0, 0);
-    }
-    return;
-  }
-  auto load_kv = [&](int blk, int st) {
+  const int tid = threadIdx.x;
+  auto issue = [&](int blk, int st) {
     mbar_arrive_expect_tx(&bar[1 + st], 2 * 8192);
-    tma_load_2d(sK + st * 8192, &tmK, &bar[1 + st], h * 64, row_base + blk * kAttnWgRows);
-    tma_load_2d(sV + st * 8192, &tmV, &bar[1 + st], h * 64, row_base + blk * kAttnWgRows);
+    load_kv(blk, sK + st * 8192, sV + st * 8192, &bar[1 + st]);
   };
   if (tid == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
     for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1);
     mbar_fence_init();
   }
   __syncthreads();
   if (tid == 0) {
     mbar_arrive_expect_tx(&bar[0], 8192);
-    tma_load_2d(sQ, &tmQ, &bar[0], h * 64, row_base + q0);
-    load_kv(0, 0);
-    if (nblk > 1) load_kv(1, 1);
+    tma_load_2d(sQ, tmQ, &bar[0], q_col, q_row);
+    issue(0, 0);
+    if (nblk > 1) issue(1, 1);
   }
-  float o[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
@@ -259,15 +94,11 @@ __global__ void __launch_bounds__(128) flash_attn_wgmma_kernel(const __grid_cons
       Wgmma<64>::mma(s, wgmma_desc_sw128(smem_u32(sQ) + k * 32), wgmma_desc_sw128(smem_u32(sK + st * 8192) + k * 32), k > 0 ? 1u : 0u);
     wgmma_commit();
     wgmma_wait<0>();
-    // ---- mask the keys past S (the block may run into the next batch or past the tensor), online softmax -------------
-    // register 4j + e: row g (e < 2) or g + 8 (e >= 2), key blk * 64 + 8j + 2 (lane % 4) + (e & 1)
-    const int key0 = blk * kAttnWgRows + 2 * (lane & 3);
+    // ---- mask, online softmax: register 4j + e is row g (e < 2) or g + 8 (e >= 2), key 8j + 2 (lane % 4) + (e & 1) of the block
+    mask(blk, s);
     float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      const int key = key0 + 8 * j;
-      if (key >= S) { s[4 * j] = -INFINITY; s[4 * j + 2] = -INFINITY; }
-      if (key + 1 >= S) { s[4 * j + 1] = -INFINITY; s[4 * j + 3] = -INFINITY; }
       mx[0] = fmaxf(mx[0], fmaxf(s[4 * j], s[4 * j + 1]));
       mx[1] = fmaxf(mx[1], fmaxf(s[4 * j + 2], s[4 * j + 3]));
     }
@@ -276,16 +107,16 @@ __global__ void __launch_bounds__(128) flash_attn_wgmma_kernel(const __grid_cons
     for (int i = 0; i < 2; ++i) {
       mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
       mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
-      m_new[i] = fmaxf(m_run[i], mx[i]);         // finite: every block holds at least one key < S
-      corr[i] = exp2f((m_run[i] - m_new[i]) * p.scale_log2);
+      m_new[i] = fmaxf(m_run[i], mx[i]);         // finite: mask leaves every row a key in every block
+      corr[i] = exp2f((m_run[i] - m_new[i]) * scale_log2);
       m_run[i] = m_new[i];
       l_run[i] *= corr[i];
     }
     uint32_t pa[4][4];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      const uint32_t lo = pack_bf16(exp2f((s[4 * j] - m_new[0]) * p.scale_log2), exp2f((s[4 * j + 1] - m_new[0]) * p.scale_log2));
-      const uint32_t hi = pack_bf16(exp2f((s[4 * j + 2] - m_new[1]) * p.scale_log2), exp2f((s[4 * j + 3] - m_new[1]) * p.scale_log2));
+      const uint32_t lo = pack_bf16(exp2f((s[4 * j] - m_new[0]) * scale_log2), exp2f((s[4 * j + 1] - m_new[0]) * scale_log2));
+      const uint32_t hi = pack_bf16(exp2f((s[4 * j + 2] - m_new[1]) * scale_log2), exp2f((s[4 * j + 3] - m_new[1]) * scale_log2));
       l_run[0] += bf16_lo(lo) + bf16_hi(lo);
       l_run[1] += bf16_lo(hi) + bf16_hi(hi);
       pa[j >> 1][(j & 1) * 2 + 0] = lo;          // A fragment of k-step j / 2: (row g, keys 2t..), (row g + 8, ...), then +8 keys
@@ -302,7 +133,7 @@ __global__ void __launch_bounds__(128) flash_attn_wgmma_kernel(const __grid_cons
     wgmma_commit();
     wgmma_wait<0>();
     __syncthreads();                             // every warp is done with stage st: refill it with block blk + 2
-    if (tid == 0 && blk + 2 < nblk) load_kv(blk + 2, st);
+    if (tid == 0 && blk + 2 < nblk) issue(blk + 2, st);
   }
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
@@ -310,13 +141,65 @@ __global__ void __launch_bounds__(128) flash_attn_wgmma_kernel(const __grid_cons
     l_run[i] += __shfl_xor_sync(0xffffffffu, l_run[i], 2);
   }
   const float inv0 = 1.0f / l_run[0], inv1 = 1.0f / l_run[1];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    o[4 * j] *= inv0;
+    o[4 * j + 1] *= inv0;
+    o[4 * j + 2] *= inv1;
+    o[4 * j + 3] *= inv1;
+  }
+}
+
+// flash_attn_wgmma_kernel: non-causal attention for any S (ViT blocks with 197 / 257 keys, the image-row prefill, 6-frame
+// video with 1182 keys, 30 x 40 VQA grids with 1201); keys past S (the block may run into the next batch or past the
+// tensor) are masked.  One CTA per (64 query rows, head, batch).
+//   kRagged (ragged image batches): batch b occupies a slot of p.S rows of which the first p.seq_lens[b] are valid; the
+//   batch is computed exactly as a uniform call with S = seq_lens[b] would compute it (the key blocks and query tiles past
+//   its length are skipped, not masked) and its output rows past that length are written as zeros.
+template <bool kRagged>
+__global__ void __launch_bounds__(128) flash_attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ,
+                                                              const __grid_constant__ CUtensorMap tmK,
+                                                              const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int h = blockIdx.y, b = blockIdx.z;
+  const int S = kRagged ? p.seq_lens[b] : p.S;
+  const int q0 = blockIdx.x * kAttnWgRows;
+  const int row_base = b * p.S;                  // rows of batch b in the [B * S, H * 64] q / k / v views
+  if (kRagged && q0 >= S) {                      // a query tile of the padding: zeros, no arithmetic
+    __nv_bfloat16* og = p.out + b * p.o_bs + h * 64;
+    for (int i = tid; i < kAttnWgRows * 8; i += 128) {
+      const int r = q0 + (i >> 3);
+      if (r < p.S) *reinterpret_cast<uint4*>(og + static_cast<long long>(r) * p.o_rs + (i & 7) * 8) = make_uint4(0, 0, 0, 0);
+    }
+    return;
+  }
+  if (tid == 0) {
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmK);
+    tma_prefetch_desc(&tmV);
+  }
+  auto load_kv = [&](int blk, uint8_t* sK, uint8_t* sV, uint64_t* bar) {
+    tma_load_2d(sK, &tmK, bar, h * 64, row_base + blk * kAttnWgRows);
+    tma_load_2d(sV, &tmV, bar, h * 64, row_base + blk * kAttnWgRows);
+  };
+  auto mask = [&](int blk, float (&s)[32]) {
+    const int key0 = blk * kAttnWgRows + 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int key = key0 + 8 * j;
+      if (key >= S) { s[4 * j] = -INFINITY; s[4 * j + 2] = -INFINITY; }
+      if (key + 1 >= S) { s[4 * j + 1] = -INFINITY; s[4 * j + 3] = -INFINITY; }
+    }
+  };
+  float o[32];
+  attn_wg_tile(&tmQ, h * 64, row_base + q0, (S + kAttnWgRows - 1) / kAttnWgRows, p.scale_log2, load_kv, mask, o);
   const int r0 = q0 + warp * 16 + (lane >> 2), r1 = r0 + 8;
   __nv_bfloat16* og = p.out + b * p.o_bs + h * 64 + 2 * (lane & 3);
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
-    if (r0 < S) *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r0) * p.o_rs + 8 * j) = pack_bf16(o[4 * j] * inv0, o[4 * j + 1] * inv0);
+    if (r0 < S) *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r0) * p.o_rs + 8 * j) = pack_bf16(o[4 * j], o[4 * j + 1]);
     else if (kRagged && r0 < p.S) *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r0) * p.o_rs + 8 * j) = 0u;
-    if (r1 < S) *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r1) * p.o_rs + 8 * j) = pack_bf16(o[4 * j + 2] * inv1, o[4 * j + 3] * inv1);
+    if (r1 < S) *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r1) * p.o_rs + 8 * j) = pack_bf16(o[4 * j + 2], o[4 * j + 3]);
     else if (kRagged && r1 < p.S) *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r1) * p.o_rs + 8 * j) = 0u;
   }
 }
@@ -325,10 +208,9 @@ __global__ void __launch_bounds__(128) flash_attn_wgmma_kernel(const __grid_cons
 // text_attn_wgmma_kernel: the text rows of a whole caption batch in one pass (caption scoring, the training-branch forward
 // of reference layers/decoder.py:916-972 through BertEncoderAsDecoder's block mask :114-137).  Text row t of caption n
 // attends to the M_b image keys of its image (image_index[n]) and to text keys 0..t of its own caption.
-//   One CTA = one warpgroup per (64 text query rows, head, caption), exactly the arithmetic of flash_attn_wgmma_kernel:
-//   the image keys come first as 64-key blocks of the image K/V cache (masked past M_b), then the caption's own text
-//   K/V blocks 0 .. q0 / 64, with the causal mask on the diagonal block only.  Text blocks past the query tile are never
-//   loaded.  A sibling of flash_attn_wgmma_kernel (same smem ring, same block step) so that kernel's code is untouched.
+//   One CTA per (64 text query rows, head, caption): the image keys come first as 64-key blocks of the image K/V cache
+//   (masked past M_b), then the caption's own text K/V blocks 0 .. q0 / 64, with the causal mask on the diagonal block
+//   only.  Text blocks past the query tile are never loaded.
 // ------------------------------------------------------------------------------------------------
 struct TextAttnParams {
   __nv_bfloat16* out;          // [N * T] rows of H * 64, row stride o_rs
@@ -346,12 +228,6 @@ __global__ void __launch_bounds__(128) text_attn_wgmma_kernel(const __grid_const
                                                              const __grid_constant__ CUtensorMap tmIK,
                                                              const __grid_constant__ CUtensorMap tmIV,
                                                              const TextAttnParams p) {
-  extern __shared__ __align__(1024) uint8_t attn_smem_raw[];
-  uint8_t* smem = attn_smem_raw + ((1024u - (smem_u32(attn_smem_raw) & 1023u)) & 1023u);
-  uint8_t* sQ = smem;
-  uint8_t* sK = smem + 8192;                     // [2 stages][64 keys][128 B]
-  uint8_t* sV = smem + 3 * 8192;
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + 5 * 8192);   // [0] Q, [1 + stage] K | V
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int h = blockIdx.y, n = blockIdx.z;
   const int q0 = blockIdx.x * kAttnWgRows;
@@ -360,51 +236,25 @@ __global__ void __launch_bounds__(128) text_attn_wgmma_kernel(const __grid_const
   const int n_img = (Mb + kAttnWgRows - 1) / kAttnWgRows;
   const int nblk = n_img + q0 / kAttnWgRows + 1;  // image blocks, then text blocks 0 .. the diagonal one
   const int trow = n * p.T;                      // rows of caption n in the [N * T, H * 64] q / k / v views
-  auto load_kv = [&](int blk, int st) {
-    mbar_arrive_expect_tx(&bar[1 + st], 2 * 8192);
-    if (blk < n_img) {
-      tma_load_2d(sK + st * 8192, &tmIK, &bar[1 + st], h * 64, img * p.M + blk * kAttnWgRows);
-      tma_load_2d(sV + st * 8192, &tmIV, &bar[1 + st], h * 64, img * p.M + blk * kAttnWgRows);
-    } else {
-      tma_load_2d(sK + st * 8192, &tmK, &bar[1 + st], h * 64, trow + (blk - n_img) * kAttnWgRows);
-      tma_load_2d(sV + st * 8192, &tmV, &bar[1 + st], h * 64, trow + (blk - n_img) * kAttnWgRows);
-    }
-  };
+  const int g0 = warp * 16 + (lane >> 2);        // tile rows of registers e < 2 (g0) and e >= 2 (g0 + 8)
   if (tid == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
     tma_prefetch_desc(&tmIK);
     tma_prefetch_desc(&tmIV);
-    for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1);
-    mbar_fence_init();
   }
-  __syncthreads();
-  if (tid == 0) {
-    mbar_arrive_expect_tx(&bar[0], 8192);
-    tma_load_2d(sQ, &tmQ, &bar[0], h * 64, trow + q0);
-    load_kv(0, 0);
-    if (nblk > 1) load_kv(1, 1);
-  }
-  float o[32];
-#pragma unroll
-  for (int i = 0; i < 32; ++i) o[i] = 0.f;
-  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
-  const int g0 = warp * 16 + (lane >> 2);        // tile rows of registers e < 2 (g0) and e >= 2 (g0 + 8)
-  mbar_wait(&bar[0], 0);
-  for (int blk = 0; blk < nblk; ++blk) {
-    const int st = blk & 1;
-    mbar_wait(&bar[1 + st], (blk >> 1) & 1);
-    float s[32];
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < 4; ++k)
-      Wgmma<64>::mma(s, wgmma_desc_sw128(smem_u32(sQ) + k * 32), wgmma_desc_sw128(smem_u32(sK + st * 8192) + k * 32), k > 0 ? 1u : 0u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    // register 4j + e: row g0 (e < 2) or g0 + 8 (e >= 2), key (of this block) 8j + 2 (lane % 4) + (e & 1)
-    const int kk0 = 2 * (lane & 3);
-    float mx[2] = {-INFINITY, -INFINITY};
+  auto load_kv = [&](int blk, uint8_t* sK, uint8_t* sV, uint64_t* bar) {
+    if (blk < n_img) {
+      tma_load_2d(sK, &tmIK, bar, h * 64, img * p.M + blk * kAttnWgRows);
+      tma_load_2d(sV, &tmIV, bar, h * 64, img * p.M + blk * kAttnWgRows);
+    } else {
+      tma_load_2d(sK, &tmK, bar, h * 64, trow + (blk - n_img) * kAttnWgRows);
+      tma_load_2d(sV, &tmV, bar, h * 64, trow + (blk - n_img) * kAttnWgRows);
+    }
+  };
+  auto mask = [&](int blk, float (&s)[32]) {
+    const int kk0 = 2 * (lane & 3);              // key (of this block) of register 4j: kk0 + 8j
     if (blk < n_img) {                           // image keys: those past M_b are masked
       const int lim = Mb - blk * kAttnWgRows;
 #pragma unroll
@@ -423,55 +273,15 @@ __global__ void __launch_bounds__(128) text_attn_wgmma_kernel(const __grid_const
         if (kk + 1 > g0 + 8) s[4 * j + 3] = -INFINITY;
       }
     }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      mx[0] = fmaxf(mx[0], fmaxf(s[4 * j], s[4 * j + 1]));
-      mx[1] = fmaxf(mx[1], fmaxf(s[4 * j + 2], s[4 * j + 3]));
-    }
-    float corr[2], m_new[2];
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
-      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
-      m_new[i] = fmaxf(m_run[i], mx[i]);         // finite: every block holds at least one visible key for every row
-      corr[i] = exp2f((m_run[i] - m_new[i]) * p.scale_log2);
-      m_run[i] = m_new[i];
-      l_run[i] *= corr[i];
-    }
-    uint32_t pa[4][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const uint32_t lo = pack_bf16(exp2f((s[4 * j] - m_new[0]) * p.scale_log2), exp2f((s[4 * j + 1] - m_new[0]) * p.scale_log2));
-      const uint32_t hi = pack_bf16(exp2f((s[4 * j + 2] - m_new[1]) * p.scale_log2), exp2f((s[4 * j + 3] - m_new[1]) * p.scale_log2));
-      l_run[0] += bf16_lo(lo) + bf16_hi(lo);
-      l_run[1] += bf16_lo(hi) + bf16_hi(hi);
-      pa[j >> 1][(j & 1) * 2 + 0] = lo;
-      pa[j >> 1][(j & 1) * 2 + 1] = hi;
-      o[4 * j] *= corr[0];
-      o[4 * j + 1] *= corr[0];
-      o[4 * j + 2] *= corr[1];
-      o[4 * j + 3] *= corr[1];
-    }
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) wgmma_m64n64k16_rs_mn(o, pa[kk], wgmma_desc_sw128(smem_u32(sV + st * 8192) + kk * 2048));
-    wgmma_commit();
-    wgmma_wait<0>();
-    __syncthreads();                             // every warp is done with stage st: refill it with block blk + 2
-    if (tid == 0 && blk + 2 < nblk) load_kv(blk + 2, st);
-  }
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    l_run[i] += __shfl_xor_sync(0xffffffffu, l_run[i], 1);
-    l_run[i] += __shfl_xor_sync(0xffffffffu, l_run[i], 2);
-  }
-  const float inv0 = 1.0f / l_run[0], inv1 = 1.0f / l_run[1];
+  };
+  float o[32];
+  attn_wg_tile(&tmQ, h * 64, trow + q0, nblk, p.scale_log2, load_kv, mask, o);
   const int r0 = q0 + g0, r1 = r0 + 8;
   __nv_bfloat16* og = p.out + static_cast<long long>(trow) * p.o_rs + h * 64 + 2 * (lane & 3);
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
-    if (r0 < p.T) *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r0) * p.o_rs + 8 * j) = pack_bf16(o[4 * j] * inv0, o[4 * j + 1] * inv0);
-    if (r1 < p.T) *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r1) * p.o_rs + 8 * j) = pack_bf16(o[4 * j + 2] * inv1, o[4 * j + 3] * inv1);
+    if (r0 < p.T) *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r0) * p.o_rs + 8 * j) = pack_bf16(o[4 * j], o[4 * j + 1]);
+    if (r1 < p.T) *reinterpret_cast<uint32_t*>(og + static_cast<long long>(r1) * p.o_rs + 8 * j) = pack_bf16(o[4 * j + 2], o[4 * j + 3]);
   }
 }
 
@@ -500,7 +310,7 @@ struct DecAttnParams {
   int chunk_rows;                  // image keys staged per TMA round (<= 512), box_rows * n_boxes
   int box_rows;                    // rows per TMA box (<= 256)
   ChainSync chain;
-  const int* img_lens;             // decode_attn_kernel<., ., true>: [B] valid image keys of each image (M = slot length;
+  const int* img_lens;             // decode_attn_kernel<., true>: [B] valid image keys of each image (M = slot length;
                                    //   chunk_rows = the staging buffer's rows, box_rows = kDecAttnRaggedBox)
 };
 
@@ -558,17 +368,16 @@ __device__ __forceinline__ void dec_attn_update(float (&sc)[4], const uint4 (&w)
 // the previous item.  128 threads = 16 key groups x 8 lanes (8 head dims each, 128-bit accesses); scores are folded
 // into per-group online-softmax states merged at the end (flash-decoding style), single pass over K and V.
 //
-// kPipe (NQ == 1 only): software pipelining of the two global-memory round trips an item used to expose -- the step's own
-// q/k/v of item k+1 are requested at the top of item k, and the text K/V rows of an item are requested before its
+// NQ == 1 (greedy decoding): software pipelining of the two global-memory round trips an item used to expose -- the step's
+// own q/k/v of item k+1 are requested at the top of item k, and the text K/V rows of an item are requested before its
 // image-key loop (shared memory) and consumed after it.  At 256 rows a CTA walks ~10 items, so the exposed latencies
 // (not the HBM stream) bounded the kernel.
 //
 // kRagged: every image has its own key count img_lens[b] (<= M, the slot length) and chunk length, so each item is
 // computed exactly as in a uniform call of its image; the CTA's chunk sequence is no longer one fixed count per item.
-template <int NQ, bool kPipe = false, bool kRagged = false>
+template <int NQ, bool kRagged = false>
 __global__ void __launch_bounds__(128)
 decode_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, const DecAttnParams p) {
-  constexpr bool kPipeOn = kPipe && NQ == 1;
   extern __shared__ uint8_t attn_dyn[];
   uint8_t* sbase = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(attn_dyn) + 127) & ~uintptr_t(127));
   const size_t kv_bytes = static_cast<size_t>(p.chunk_rows) * 128;  // one of K / V of one unit
@@ -673,7 +482,7 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
     }
   }
 
-  // kPipe: (q, k | v) of the NEXT item, requested one item ahead
+  // NQ == 1: (q, k | v) of the NEXT item, requested one item ahead
   float nxt_a = 0.f, nxt_b = 0.f;
   auto request_qkv = [&](int k, float& a, float& b2) {
     if (k < n_my) {
@@ -688,7 +497,7 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
       }
     }
   };
-  if (kPipeOn) request_qkv(kPre, nxt_a, nxt_b);   // items 0..kPre-1 were requested above
+  if (NQ == 1) request_qkv(kPre, nxt_a, nxt_b);   // items 0..kPre-1 were requested above
 
   int u_base = 0;                 // units of the items before this one
   for (int k = 0; k < n_my; ++k) {
@@ -698,7 +507,7 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
     const int crows = kRagged ? dec_attn_chunk_rows(Mb) : p.chunk_rows;
     const int nch = kRagged ? (Mb + crows - 1) / crows : n_chunks;
     float cur_a = 0.f, cur_b = 0.f;
-    if (kPipeOn && k >= kPre) {
+    if (NQ == 1 && k >= kPre) {
       cur_a = nxt_a;
       cur_b = nxt_b;
       request_qkv(k + 1, nxt_a, nxt_b);
@@ -710,13 +519,13 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
       const float* bias = p.bqkv + h * 64;
       const bool have = (NQ == 1) && (k < kPre);
       if (tid < 64) {
-        const float qv = have ? pre_a[k < kPre ? k : 0] : (kPipeOn ? cur_a : ld_partials(row + tid, p.n_partials, p.partial_stride));
-        const float kv = have ? pre_b[k < kPre ? k : 0] : (kPipeOn ? cur_b : ld_partials(row + D + tid, p.n_partials, p.partial_stride));
+        const float qv = have ? pre_a[k < kPre ? k : 0] : (NQ == 1 ? cur_a : ld_partials(row + tid, p.n_partials, p.partial_stride));
+        const float kv = have ? pre_b[k < kPre ? k : 0] : (NQ == 1 ? cur_b : ld_partials(row + D + tid, p.n_partials, p.partial_stride));
         q_s[qi][tid] = (qv + bias[tid]) * 0.125f;
         p.txt_k[(static_cast<long long>(r) * p.T_alloc + pos) * D + h * 64 + tid] = __float2bfloat16_rn(kv + bias[D + tid]);
       } else {
         const int d = tid - 64;
-        const float vv = have ? pre_a[k < kPre ? k : 0] : (kPipeOn ? cur_a : ld_partials(row + 2 * D + d, p.n_partials, p.partial_stride));
+        const float vv = have ? pre_a[k < kPre ? k : 0] : (NQ == 1 ? cur_a : ld_partials(row + 2 * D + d, p.n_partials, p.partial_stride));
         p.txt_v[(static_cast<long long>(r) * p.T_alloc + pos) * D + h * 64 + d] = __float2bfloat16_rn(vv + bias[2 * D + d]);
       }
     }
@@ -766,8 +575,8 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
       }
       dec_attn_update(sc, w, m_run[qi], l_run[qi], acc[qi]);
     };
-    uint4 tu[4], tw[4];                       // kPipe: text positions 0..63 of this item, in flight across the image loop
-    if (kPipeOn) {
+    uint4 tu[4], tw[4];                       // NQ == 1: text positions 0..63 of this item, in flight across the image loop
+    if (NQ == 1) {
       text_chunk_load(b, 0, tu, tw);
     } else {
 #pragma unroll
@@ -819,7 +628,7 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
       if (tid == 0 && u_idx + 2 < n_units) issue_unit(u_idx + 2);
     }
     u_base += nch;
-    if (kPipeOn) {
+    if (NQ == 1) {
       text_chunk_use(0, 0, tu, tw);
       for (int base = 64; base < n_txt; base += 64) {   // captions longer than 64 tokens: the rest the plain way
         uint4 u[4], w[4];
@@ -895,100 +704,12 @@ __device__ __forceinline__ void store_split3_pair(__nv_bfloat16* row, int d_mode
   *reinterpret_cast<uint32_t*>(row + 2 * d_model + col) = hi;
 }
 
-__global__ void __launch_bounds__(128) attn_f32_kernel(const AttnF32Params p) {
-  extern __shared__ float attn_f32_smem[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  float* q_s = attn_f32_smem + warp * (64 + p.S);
-  float* sc = q_s + 64;
-  const long long item = static_cast<long long>(blockIdx.x) * 4 + warp;
-  const long long total = static_cast<long long>(p.B) * p.H * p.S;
-  if (item >= total) return;
-  const int row = static_cast<int>(item % p.S);
-  const int h = static_cast<int>((item / p.S) % p.H);
-  const int b = static_cast<int>(item / (static_cast<long long>(p.S) * p.H));
-  const int S = p.seq_lens != nullptr ? p.seq_lens[b] : p.S;
-  if (row >= S) {
-    store_split3_pair(p.out + b * p.o_bs + static_cast<long long>(row) * 3 * p.d_model, p.d_model, h * 64 + 2 * lane, 0.f, 0.f);
-    return;
-  }
-  const float* qg = p.q + b * p.q_bs + static_cast<long long>(row) * p.q_rs + h * 64;
-  const float* kg = p.k + b * p.kv_bs + h * 64;
-  const float* vg = p.v + b * p.kv_bs + h * 64;
-  q_s[lane] = qg[lane] * 0.125f;             // Q / sqrt(64) before the product (reference layers/bert/modeling_bert.py:42-43)
-  q_s[lane + 32] = qg[lane + 32] * 0.125f;
-  __syncwarp();
-  float mx = -INFINITY;
-  for (int j0 = 0; j0 < S; j0 += 32) {
-    const int j = j0 + lane;
-    if (j < S) {
-      const float4* kr = reinterpret_cast<const float4*>(kg + static_cast<long long>(j) * p.kv_rs);
-      float a = 0.f;
-#pragma unroll
-      for (int d = 0; d < 16; ++d) {
-        const float4 kk = kr[d];
-        a = fmaf(q_s[4 * d], kk.x, a); a = fmaf(q_s[4 * d + 1], kk.y, a);
-        a = fmaf(q_s[4 * d + 2], kk.z, a); a = fmaf(q_s[4 * d + 3], kk.w, a);
-      }
-      sc[j] = a;
-      mx = fmaxf(mx, a);
-    }
-  }
-  mx = warp_max(mx);
-  float sum = 0.f;
-  for (int j = lane; j < S; j += 32) {
-    const float e = expf(sc[j] - mx);
-    sc[j] = e;
-    sum += e;
-  }
-  sum = warp_sum(sum);
-  __syncwarp();
-  float a0 = 0.f, a1 = 0.f;
-  for (int j = 0; j < S; ++j) {
-    const float2 vv = *reinterpret_cast<const float2*>(vg + static_cast<long long>(j) * p.kv_rs + 2 * lane);
-    a0 = fmaf(sc[j], vv.x, a0);
-    a1 = fmaf(sc[j], vv.y, a1);
-  }
-  __nv_bfloat16* orow = p.out + b * p.o_bs + static_cast<long long>(row) * 3 * p.d_model;
-  store_split3_pair(orow, p.d_model, h * 64 + 2 * lane, a0 / sum, a1 / sum);
-}
-
-// Parity-mode sibling of text_attn_wgmma_kernel: plain fp32, one warp per (caption, head, text row); q / k / v fp32 rows of
-// d_model elements ([N * T] text rows, [B * M] image rows), output rows in the split format [hi | lo | hi] (3 * d_model).
-struct TextAttnF32Params {
-  const float* q;
-  const float* k;                // text K / V [N * T, d_model]
-  const float* v;
-  const float* img_k;            // image K / V [B * M, d_model]
-  const float* img_v;
-  __nv_bfloat16* out;            // [N * T, 3 * d_model]
-  int N, T, H, d_model, M;
-  const int* img_lens;           // null or [B]
-  const int* image_index;        // null or [N]
-};
-
-__global__ void __launch_bounds__(128) text_attn_f32_kernel(const TextAttnF32Params p) {
-  extern __shared__ float attn_f32_smem[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  float* q_s = attn_f32_smem + warp * (64 + p.M + p.T);
-  float* sc = q_s + 64;
-  const long long item = static_cast<long long>(blockIdx.x) * 4 + warp;
-  const long long total = static_cast<long long>(p.N) * p.H * p.T;
-  if (item >= total) return;
-  const int t = static_cast<int>(item % p.T);
-  const int h = static_cast<int>((item / p.T) % p.H);
-  const int n = static_cast<int>(item / (static_cast<long long>(p.T) * p.H));
-  const int img = p.image_index != nullptr ? p.image_index[n] : n;
-  const int Mb = p.img_lens != nullptr ? p.img_lens[img] : p.M;
-  const int n_keys = Mb + t + 1;
-  const long long trow = static_cast<long long>(n) * p.T;
-  const float* qg = p.q + (trow + t) * p.d_model + h * 64;
-  auto key_row = [&](int j, bool want_v) -> const float* {
-    if (j < Mb) return (want_v ? p.img_v : p.img_k) + (static_cast<long long>(img) * p.M + j) * p.d_model + h * 64;
-    return (want_v ? p.v : p.k) + (trow + j - Mb) * p.d_model + h * 64;
-  };
-  q_s[lane] = qg[lane] * 0.125f;             // Q / sqrt(64) before the product (reference layers/bert/modeling_bert.py:42-43)
-  q_s[lane + 32] = qg[lane + 32] * 0.125f;
-  __syncwarp();
+// One query row on one warp: softmax(q k^T) v over n_keys keys in plain fp32.  q_s: the row's q, already scaled by 1/8
+// (64 floats in shared memory, visible to the warp); sc: n_keys floats of score scratch; key_row(j, want_v): the 64 fp32
+// of key j's K (false) or V (true), 16-byte aligned.  Returns output dims 2 * lane and 2 * lane + 1.
+template <class KeyRow>
+__device__ __forceinline__ float2 attn_row_f32(const float* q_s, float* sc, int n_keys, const KeyRow& key_row) {
+  const int lane = threadIdx.x & 31;
   float mx = -INFINITY;
   for (int j0 = 0; j0 < n_keys; j0 += 32) {
     const int j = j0 + lane;
@@ -1020,7 +741,71 @@ __global__ void __launch_bounds__(128) text_attn_f32_kernel(const TextAttnF32Par
     a0 = fmaf(sc[j], vv.x, a0);
     a1 = fmaf(sc[j], vv.y, a1);
   }
-  store_split3_pair(p.out + (trow + t) * 3 * p.d_model, p.d_model, h * 64 + 2 * lane, a0 / sum, a1 / sum);
+  return make_float2(a0 / sum, a1 / sum);
+}
+
+__global__ void __launch_bounds__(128) attn_f32_kernel(const AttnF32Params p) {
+  extern __shared__ __align__(16) float attn_f32_smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* q_s = attn_f32_smem + warp * (64 + p.S);
+  const long long item = static_cast<long long>(blockIdx.x) * 4 + warp;
+  const long long total = static_cast<long long>(p.B) * p.H * p.S;
+  if (item >= total) return;
+  const int row = static_cast<int>(item % p.S);
+  const int h = static_cast<int>((item / p.S) % p.H);
+  const int b = static_cast<int>(item / (static_cast<long long>(p.S) * p.H));
+  const int S = p.seq_lens != nullptr ? p.seq_lens[b] : p.S;
+  __nv_bfloat16* orow = p.out + b * p.o_bs + static_cast<long long>(row) * 3 * p.d_model;
+  if (row >= S) {
+    store_split3_pair(orow, p.d_model, h * 64 + 2 * lane, 0.f, 0.f);
+    return;
+  }
+  const float* qg = p.q + b * p.q_bs + static_cast<long long>(row) * p.q_rs + h * 64;
+  q_s[lane] = qg[lane] * 0.125f;             // Q / sqrt(64) before the product (reference layers/bert/modeling_bert.py:42-43)
+  q_s[lane + 32] = qg[lane + 32] * 0.125f;
+  __syncwarp();
+  const float2 r = attn_row_f32(q_s, q_s + 64, S, [&](int j, bool want_v) {
+    return (want_v ? p.v : p.k) + b * p.kv_bs + static_cast<long long>(j) * p.kv_rs + h * 64;
+  });
+  store_split3_pair(orow, p.d_model, h * 64 + 2 * lane, r.x, r.y);
+}
+
+// Parity-mode sibling of text_attn_wgmma_kernel: plain fp32, one warp per (caption, head, text row); q / k / v fp32 rows of
+// d_model elements ([N * T] text rows, [B * M] image rows), output rows in the split format [hi | lo | hi] (3 * d_model).
+struct TextAttnF32Params {
+  const float* q;
+  const float* k;                // text K / V [N * T, d_model]
+  const float* v;
+  const float* img_k;            // image K / V [B * M, d_model]
+  const float* img_v;
+  __nv_bfloat16* out;            // [N * T, 3 * d_model]
+  int N, T, H, d_model, M;
+  const int* img_lens;           // null or [B]
+  const int* image_index;        // null or [N]
+};
+
+__global__ void __launch_bounds__(128) text_attn_f32_kernel(const TextAttnF32Params p) {
+  extern __shared__ __align__(16) float attn_f32_smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* q_s = attn_f32_smem + warp * (64 + p.M + p.T);
+  const long long item = static_cast<long long>(blockIdx.x) * 4 + warp;
+  const long long total = static_cast<long long>(p.N) * p.H * p.T;
+  if (item >= total) return;
+  const int t = static_cast<int>(item % p.T);
+  const int h = static_cast<int>((item / p.T) % p.H);
+  const int n = static_cast<int>(item / (static_cast<long long>(p.T) * p.H));
+  const int img = p.image_index != nullptr ? p.image_index[n] : n;
+  const int Mb = p.img_lens != nullptr ? p.img_lens[img] : p.M;
+  const long long trow = static_cast<long long>(n) * p.T;
+  const float* qg = p.q + (trow + t) * p.d_model + h * 64;
+  q_s[lane] = qg[lane] * 0.125f;             // Q / sqrt(64) before the product (reference layers/bert/modeling_bert.py:42-43)
+  q_s[lane + 32] = qg[lane + 32] * 0.125f;
+  __syncwarp();
+  const float2 r = attn_row_f32(q_s, q_s + 64, Mb + t + 1, [&](int j, bool want_v) {   // image keys, then text keys 0..t
+    if (j < Mb) return (want_v ? p.img_v : p.img_k) + (static_cast<long long>(img) * p.M + j) * p.d_model + h * 64;
+    return (want_v ? p.v : p.k) + (trow + j - Mb) * p.d_model + h * 64;
+  });
+  store_split3_pair(p.out + (trow + t) * 3 * p.d_model, p.d_model, h * 64 + 2 * lane, r.x, r.y);
 }
 
 struct DecAttnF32Params {
@@ -1041,9 +826,13 @@ struct DecAttnF32Params {
   const int* img_lens;            // null, or [B] valid image keys of each image (ragged batches; M is the slot length)
 };
 
+// Shared memory of one warp of decode_attn_f32_kernel in floats: q | k | v of the new token, then the scores; a multiple
+// of 4 so that every warp's k / v rows are 16-byte aligned.
+__host__ __device__ __forceinline__ int dec_attn_f32_warp_floats(int M, int T_alloc) { return (192 + M + T_alloc + 3) & ~3; }
+
 // one warp per (sequence r, head h); 4 warps per CTA
 __global__ void __launch_bounds__(128) decode_attn_f32_kernel(const DecAttnF32Params p) {
-  extern __shared__ float attn_f32_smem[];
+  extern __shared__ __align__(16) float attn_f32_smem[];
   griddep_launch_early();
   bool finished;
   if (p.chain.counters != nullptr) {
@@ -1057,10 +846,9 @@ __global__ void __launch_bounds__(128) decode_attn_f32_kernel(const DecAttnF32Pa
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int D = p.D, H = D / 64;
   const int pos = (p.state != nullptr) ? p.state->pos : p.pos_fixed;
-  float* q_s = attn_f32_smem + warp * (192 + p.M + p.T_alloc);
+  float* q_s = attn_f32_smem + warp * dec_attn_f32_warp_floats(p.M, p.T_alloc);
   float* k_s = q_s + 64;
   float* v_s = q_s + 128;
-  float* sc = q_s + 192;
   const int item = blockIdx.x * 4 + warp;
   if (item < p.R * H) {
     const int r = item / H, h = item - r * H;
@@ -1079,51 +867,15 @@ __global__ void __launch_bounds__(128) decode_attn_f32_kernel(const DecAttnF32Pa
       p.txt_v[(static_cast<long long>(r) * p.T_alloc + pos) * D + h * 64 + d] = vn;
     }
     __syncwarp();
-    auto key_ptr = [&](int j, bool want_v) -> const float* {   // row of key j (j != newest)
+    // image keys, then text positions 0..pos-1 through src_row, then the new token from shared memory
+    const float2 o = attn_row_f32(q_s, q_s + 192, n_keys, [&](int j, bool want_v) -> const float* {
+      if (j == n_keys - 1) return want_v ? v_s : k_s;
       if (j < Mb) return (want_v ? p.img_v : p.img_k) + (static_cast<long long>(b) * p.M + j) * D + h * 64;
       const int t = j - Mb;
       const int pr = (p.src_row != nullptr) ? p.src_row[r * p.T_alloc + t] : r;
       return (want_v ? p.txt_v : p.txt_k) + (static_cast<long long>(pr) * p.T_alloc + t) * D + h * 64;
-    };
-    float mx = -INFINITY;
-    for (int j0 = 0; j0 < n_keys; j0 += 32) {
-      const int j = j0 + lane;
-      if (j < n_keys) {
-        float a = 0.f;
-        if (j == n_keys - 1) {
-#pragma unroll
-          for (int d = 0; d < 64; ++d) a = fmaf(q_s[d], k_s[d], a);
-        } else {
-          const float4* kr = reinterpret_cast<const float4*>(key_ptr(j, false));
-#pragma unroll
-          for (int d = 0; d < 16; ++d) {
-            const float4 kk = kr[d];
-            a = fmaf(q_s[4 * d], kk.x, a); a = fmaf(q_s[4 * d + 1], kk.y, a);
-            a = fmaf(q_s[4 * d + 2], kk.z, a); a = fmaf(q_s[4 * d + 3], kk.w, a);
-          }
-        }
-        sc[j] = a;
-        mx = fmaxf(mx, a);
-      }
-    }
-    mx = warp_max(mx);
-    float sum = 0.f;
-    for (int j = lane; j < n_keys; j += 32) {
-      const float e = expf(sc[j] - mx);
-      sc[j] = e;
-      sum += e;
-    }
-    sum = warp_sum(sum);
-    __syncwarp();
-    float a0 = 0.f, a1 = 0.f;
-    for (int j = 0; j + 1 < n_keys; ++j) {
-      const float2 vv = *reinterpret_cast<const float2*>(key_ptr(j, true) + 2 * lane);
-      a0 = fmaf(sc[j], vv.x, a0);
-      a1 = fmaf(sc[j], vv.y, a1);
-    }
-    a0 = fmaf(sc[n_keys - 1], v_s[2 * lane], a0);
-    a1 = fmaf(sc[n_keys - 1], v_s[2 * lane + 1], a1);
-    store_split3_pair(p.ctx + static_cast<long long>(r) * 3 * D, D, h * 64 + 2 * lane, a0 / sum, a1 / sum);
+    });
+    store_split3_pair(p.ctx + static_cast<long long>(r) * 3 * D, D, h * 64 + 2 * lane, o.x, o.y);
   }
   chain_signal(p.chain);
 }

@@ -25,6 +25,7 @@
 #include <cstdio>
 #include <cstring>
 #include <map>
+#include <mutex>
 #include <set>
 #include <string>
 #include <utility>
@@ -467,14 +468,26 @@ static LnParams ln_params(const float* x, const float* bias, const float* resid,
   return p;
 }
 
-template <int NW>
-static void launch_flash(const AttnParams& p, cudaStream_t st) {
-  dim3 grid((p.S + NW * 16 - 1) / (NW * 16), p.H, p.B);
-  flash_attn_kernel<NW><<<grid, NW * 32, 0, st>>>(p);
+// Raises `kernel`'s dynamic shared-memory limit to smem bytes on the engine's device; the attribute is set once per kernel,
+// device and larger size (the parity and decode attention kernels size their shared memory per call).
+static int set_dyn_smem(gitb200_engine* h, const void* kernel, size_t smem) {
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, size_t> done;
+  std::lock_guard<std::mutex> lock(mu);
+  size_t& have = done[{kernel, h->device}];
+  if (have < smem) {
+    CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+    have = smem;
+  }
+  return 0;
 }
-// Hopper attention (attention.cuh: flash_attn_wgmma_kernel) for batches stored back to back (row b * S + i of the q / k / v
-// views), which is every ViT and prefill call; TMA needs the row pitch and the bases 16-byte aligned (get_tmap checks).
-static int launch_attention_wgmma(gitb200_engine* h, const AttnParams& ap, cudaStream_t st) {
+
+// Non-causal attention (attention.cuh: flash_attn_wgmma_kernel) for batches stored back to back (row b * S + i of the
+// q / k / v views), which is every ViT and prefill call; TMA needs the row pitch and the bases 16-byte aligned (get_tmap
+// checks).
+static int launch_attention(gitb200_engine* h, const AttnParams& ap, cudaStream_t st) {
+  if (ap.q_bs != static_cast<long long>(ap.S) * ap.q_rs || ap.kv_bs != static_cast<long long>(ap.S) * ap.kv_rs)
+    return fail(h, "attention: batches must be stored back to back (batch stride = S * row stride)");
   AttnParams p = ap;
   p.scale_log2 = 0.125f * 1.44269504088896340736f;
   const long long rows = static_cast<long long>(ap.B) * ap.S;
@@ -489,40 +502,10 @@ static int launch_attention_wgmma(gitb200_engine* h, const AttnParams& ap, cudaS
   return 0;
 }
 
-static int launch_attention(gitb200_engine* h, const AttnParams& ap, cudaStream_t st) {
-  if (ap.q_bs == static_cast<long long>(ap.S) * ap.q_rs && ap.kv_bs == static_cast<long long>(ap.S) * ap.kv_rs)
-    return launch_attention_wgmma(h, ap, st);
-  if (ap.seq_lens != nullptr) return fail(h, "attention: per-batch lengths need batches stored back to back");
-  // flash_attn_kernel: batches with other strides
-  AttnParams p = ap;
-  p.scale_log2 = 0.125f * 1.44269504088896340736f;
-  // query rows per CTA = 16 * NW: least padding first, then the larger tile (K/V are re-read per query tile)
-  const int cands[4] = {8, 7, 6, 4};
-  int best = 4;
-  long long best_pad = 1LL << 60;
-  for (int i = 0; i < 4; ++i) {
-    const int rows = cands[i] * 16;
-    const long long padded = static_cast<long long>((p.S + rows - 1) / rows) * rows;
-    if (padded < best_pad) { best_pad = padded; best = cands[i]; }
-  }
-  switch (best) {
-    case 8: launch_flash<8>(p, st); break;
-    case 7: launch_flash<7>(p, st); break;
-    case 6: launch_flash<6>(p, st); break;
-    default: launch_flash<4>(p, st); break;
-  }
-  CKL(h, "flash_attn_kernel");
-  return 0;
-}
-
 static int launch_attention_f32(gitb200_engine* h, const AttnF32Params& p, cudaStream_t st) {
   const size_t smem = static_cast<size_t>(4) * (64 + p.S) * sizeof(float);
   if (smem > 200 * 1024) return fail(h, "parity attention: %d keys do not fit in shared memory", p.S);
-  static size_t attr_done[64] = {0};
-  if (attr_done[h->device & 63] < smem) {
-    CK(cudaFuncSetAttribute(attn_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    attr_done[h->device & 63] = smem;
-  }
+  TRY(set_dyn_smem(h, reinterpret_cast<const void*>(attn_f32_kernel), smem));
   const long long items = static_cast<long long>(p.B) * p.H * p.S;
   attn_f32_kernel<<<static_cast<unsigned int>((items + 3) / 4), 128, smem, st>>>(p);
   CKL(h, "attn_f32_kernel");
@@ -551,11 +534,7 @@ static int launch_text_attention(gitb200_engine* h, const bf16* q, const bf16* k
 static int launch_text_attention_f32(gitb200_engine* h, const TextAttnF32Params& p, cudaStream_t st) {
   const size_t smem = static_cast<size_t>(4) * (64 + p.M + p.T) * sizeof(float);
   if (smem > 200 * 1024) return fail(h, "parity text attention: %d keys do not fit in shared memory", p.M + p.T);
-  static size_t attr_done[64] = {0};
-  if (attr_done[h->device & 63] < smem) {
-    CK(cudaFuncSetAttribute(text_attn_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    attr_done[h->device & 63] = smem;
-  }
+  TRY(set_dyn_smem(h, reinterpret_cast<const void*>(text_attn_f32_kernel), smem));
   const long long items = static_cast<long long>(p.N) * p.H * p.T;
   text_attn_f32_kernel<<<static_cast<unsigned int>((items + 3) / 4), 128, smem, st>>>(p);
   CKL(h, "text_attn_f32_kernel");
@@ -589,19 +568,15 @@ static DecAttnGeom dec_attn_geometry(int M, const int* lens, int n, int num_sms,
   return g;
 }
 
-template <int NQ, bool kPipe, bool kRagged>
+template <int NQ, bool kRagged>
 static int launch_decode_attn_inst(gitb200_engine* h, const DecAttnParams& ap, int grid, size_t smem, bool pdl,
                                    cudaStream_t st, const CUtensorMap& tk, const CUtensorMap& tv) {
-  static size_t attr_done[64] = {0};
-  if (attr_done[h->device & 63] < smem) {
-    CK(cudaFuncSetAttribute(decode_attn_kernel<NQ, kPipe, kRagged>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    attr_done[h->device & 63] = smem;
-  }
-  CK(launch_k(pdl, decode_attn_kernel<NQ, kPipe, kRagged>, dim3(grid), dim3(128), smem, st, tk, tv, ap));
+  TRY(set_dyn_smem(h, reinterpret_cast<const void*>(decode_attn_kernel<NQ, kRagged>), smem));
+  CK(launch_k(pdl, decode_attn_kernel<NQ, kRagged>, dim3(grid), dim3(128), smem, st, tk, tv, ap));
   CKL(h, "decode_attn_kernel");
   return 0;
 }
-// decode_attn_kernel<beam, beam == 1, ragged> on `grid` CTAs; ap.chunk_rows / box_rows and smem from dec_attn_geometry.
+// decode_attn_kernel<beam, ragged> on `grid` CTAs; ap.chunk_rows / box_rows and smem from dec_attn_geometry.
 static int launch_decode_attn(gitb200_engine* h, const DecAttnParams& ap, int beam, int grid, size_t smem, bool pdl,
                               cudaStream_t st) {
   CUtensorMap tk, tv;
@@ -609,23 +584,23 @@ static int launch_decode_attn(gitb200_engine* h, const DecAttnParams& ap, int be
   TRY(get_tmap(h, ap.img_v, static_cast<long long>(ap.B) * ap.M, ap.D, ap.D, ap.box_rows, &tv, false));
   const bool rg = ap.img_lens != nullptr;
   switch (beam) {
-    case 1: return rg ? launch_decode_attn_inst<1, true, true>(h, ap, grid, smem, pdl, st, tk, tv)
-                      : launch_decode_attn_inst<1, true, false>(h, ap, grid, smem, pdl, st, tk, tv);
-    case 2: return rg ? launch_decode_attn_inst<2, false, true>(h, ap, grid, smem, pdl, st, tk, tv)
-                      : launch_decode_attn_inst<2, false, false>(h, ap, grid, smem, pdl, st, tk, tv);
-    case 3: return rg ? launch_decode_attn_inst<3, false, true>(h, ap, grid, smem, pdl, st, tk, tv)
-                      : launch_decode_attn_inst<3, false, false>(h, ap, grid, smem, pdl, st, tk, tv);
-    case 4: return rg ? launch_decode_attn_inst<4, false, true>(h, ap, grid, smem, pdl, st, tk, tv)
-                      : launch_decode_attn_inst<4, false, false>(h, ap, grid, smem, pdl, st, tk, tv);
+    case 1: return rg ? launch_decode_attn_inst<1, true>(h, ap, grid, smem, pdl, st, tk, tv)
+                      : launch_decode_attn_inst<1, false>(h, ap, grid, smem, pdl, st, tk, tv);
+    case 2: return rg ? launch_decode_attn_inst<2, true>(h, ap, grid, smem, pdl, st, tk, tv)
+                      : launch_decode_attn_inst<2, false>(h, ap, grid, smem, pdl, st, tk, tv);
+    case 3: return rg ? launch_decode_attn_inst<3, true>(h, ap, grid, smem, pdl, st, tk, tv)
+                      : launch_decode_attn_inst<3, false>(h, ap, grid, smem, pdl, st, tk, tv);
+    case 4: return rg ? launch_decode_attn_inst<4, true>(h, ap, grid, smem, pdl, st, tk, tv)
+                      : launch_decode_attn_inst<4, false>(h, ap, grid, smem, pdl, st, tk, tv);
     default: return fail(h, "decode: beam size %d not supported (1 .. 4)", beam);
   }
 }
 
 // decode_attn_f32_kernel (parity mode): one warp per (sequence, head); *ctas receives the grid.
 static int launch_decode_attn_f32(gitb200_engine* h, const DecAttnF32Params& ap, bool pdl, cudaStream_t st, unsigned int* ctas) {
-  const size_t smem = static_cast<size_t>(4) * (192 + ap.M + ap.T_alloc) * sizeof(float);
+  const size_t smem = static_cast<size_t>(4) * dec_attn_f32_warp_floats(ap.M, ap.T_alloc) * sizeof(float);
   if (smem > 200 * 1024) return fail(h, "parity decode attention: %d keys do not fit in shared memory", ap.M + ap.T_alloc);
-  CK(cudaFuncSetAttribute(decode_attn_f32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  TRY(set_dyn_smem(h, reinterpret_cast<const void*>(decode_attn_f32_kernel), smem));
   *ctas = static_cast<unsigned int>((ap.R * (ap.D / 64) + 3) / 4);
   CK(launch_k(pdl, decode_attn_f32_kernel, dim3(*ctas), dim3(128), smem, st, ap));
   CKL(h, "decode_attn_f32_kernel");

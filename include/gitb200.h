@@ -220,21 +220,22 @@ int gitb200_op_gemm(const void* a_dev, const void* w_dev, const float* bias_dev,
 int gitb200_op_layernorm(const float* x_dev, const float* bias_dev, const float* resid_dev, const float* gamma_dev,
                          const float* beta_dev, float eps, float* out_f32_dev, void* out_bf16_dev, int rows, int D,
                          void* stream);
-/* Non-causal multi-head attention over packed bf16 rows: q/k/v [B, S, H*64] with the given row strides
- * (elements) and batch strides; out bf16 [B, S, H*64]. softmax(q k^T / 8) v. */
+/* Non-causal multi-head attention over packed bf16 rows: q/k/v [B, S, H*64] with the given row strides (elements);
+ * batches are stored back to back (q_batch_stride = S * q_row_stride, kv_batch_stride = S * kv_row_stride; other batch
+ * strides are refused); out bf16 [B, S, H*64] with its own row and batch strides. softmax(q k^T / 8) v. */
 int gitb200_op_attention(const void* q_dev, const void* k_dev, const void* v_dev, void* out_dev, int B, int S, int H,
                          long long q_row_stride, long long kv_row_stride, long long q_batch_stride,
                          long long kv_batch_stride, long long out_row_stride, long long out_batch_stride,
                          void* stream);
-/* gitb200_op_attention plus per-batch lengths and parity mode.  seq_lens_host: NULL or B lengths in 1..S (ragged: batches
- * must be stored back to back; batch b is computed as a call with S = seq_lens[b] and its rows past that length are
+/* gitb200_op_attention plus per-batch lengths and parity mode.  seq_lens_host: NULL or B lengths in 1..S (ragged: batch b
+ * is computed as a call with S = seq_lens[b] and its rows past that length are
  * zeros).  fp32 != 0: attn_f32_kernel on fp32 q/k/v; output rows are 3*H*64 bf16 [hi | lo | hi], out_row_stride is
  * ignored. */
 int gitb200_op_attention_ex(const void* q_dev, const void* k_dev, const void* v_dev, void* out_dev, int B, int S, int H,
                             long long q_row_stride, long long kv_row_stride, long long q_batch_stride,
                             long long kv_batch_stride, long long out_row_stride, long long out_batch_stride,
                             const int32_t* seq_lens_host, int fp32, void* stream);
-/* One layer's decode-step attention as the kernel chain runs it: decode_attn_kernel<beam, beam == 1, img_lens != NULL>,
+/* One layer's decode-step attention as the kernel chain runs it: decode_attn_kernel<beam, img_lens != NULL>,
  * or decode_attn_f32_kernel when fp32 != 0.
  * qkv_dev: n_partials (1..4) fp32 split-K partial buffers [B*beam, 3*D], B*beam*3*D elements apart; bqkv_dev fp32 [3*D].
  * img_k/v_dev [B, M, D] and txt_k/v_dev [B*beam, T_alloc, D]: bf16, or fp32 when fp32 != 0.  Position pos of every text

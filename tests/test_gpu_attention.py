@@ -1,9 +1,8 @@
 """Every attention kernel through a C-ABI op entry point against a plain fp64 PyTorch statement of the same operation.
 
 Kernels (csrc/attention.cuh) and their entry points:
-  gitb200_op_decode_attention: decode_attn_kernel<beam, beam == 1, ragged> and decode_attn_f32_kernel (parity mode);
-  gitb200_op_attention_ex: flash_attn_wgmma_kernel<false / true>, flash_attn_kernel<NW> (batches that are not stored back
-  to back) and attn_f32_kernel (parity mode).
+  gitb200_op_decode_attention: decode_attn_kernel<beam, ragged> and decode_attn_f32_kernel (parity mode);
+  gitb200_op_attention_ex: flash_attn_wgmma_kernel<false / true> and attn_f32_kernel (parity mode).
 
 Random data alone lets a dropped key hide inside the tolerance, so every case plants keys: for some (row, head) pairs
 one key at a boundary of the kernel (the last valid key, the first and last key of each 64-key block or decode chunk,
@@ -23,7 +22,6 @@ import torch
 TOL_DECODE = 5.5e-3       # decode_attn_kernel: fp32 softmax, bf16 output; observed 1.58e-3
 TOL_DECODE_F32 = 1e-5     # decode_attn_f32_kernel: fp32, output hi + lo; observed 2.84e-6
 TOL_WGMMA = 3.5e-3        # flash_attn_wgmma_kernel: bf16 P, bf16 output; observed 9.11e-4
-TOL_MMA = 6e-3            # flash_attn_kernel: bf16 P, bf16 output; observed 1.77e-3
 TOL_ATTN_F32 = 7e-6       # attn_f32_kernel: fp32, output hi + lo; observed 1.90e-6
 ABS = 1e-5
 PAD = 3e4                 # a large finite value in rows no valid row may read
@@ -240,8 +238,6 @@ def make_attention_case(B, S, H, lens=None, fp32=False, seed=0, pad=PAD, tol=TOL
 
 
 WGMMA_RAGGED_LENS = [2, 63, 64, 65, 128, 197, 1201]
-# flash_attn_kernel<NW> takes 16 * NW query rows per CTA, NW in (8, 7, 6, 4) with the least padding
-STRIDED_S = [(128, 8), (112, 7), (96, 6), (64, 4), (197, 7), (1201, 4)]
 F32_ATTN_CASES = [(2, 197, 2, None), (3, 1201, 2, [2, 65, 1201])]
 UNIFORM_CASES = [(2, 197, 12), (1, 1201, 2)]
 
@@ -252,10 +248,6 @@ def _wgmma_ragged_case(pad=PAD):
 
 def _uniform_case(B, S, H):
     return make_attention_case(B, S, H, seed=12)
-
-
-def _strided_case(S, nw):
-    return make_attention_case(2, S, 2, seed=13 + S, tol=TOL_MMA)
 
 
 def _f32_attn_case(B, S, H, lens, pad=PAD):
@@ -318,13 +310,13 @@ def test_ragged_decode_case_sensitivity(beam):
     assert _ragged_case(beam)['n_plants'] >= 6 * 4
 
 
-@pytest.mark.parametrize('build', ['wgmma_ragged', 'uniform', 'strided', 'f32'])
+@pytest.mark.parametrize('build', ['wgmma_ragged', 'uniform', 'f32'])
 def test_attention_case_sensitivity(build):
     """Every GPU attention case, built: each planted key moves its row by at least 4x the tolerance."""
     if build == 'wgmma_ragged':
         _wgmma_ragged_case()
-    for args in {'uniform': UNIFORM_CASES, 'strided': STRIDED_S, 'f32': F32_ATTN_CASES, 'wgmma_ragged': []}[build]:
-        {'uniform': _uniform_case, 'strided': _strided_case, 'f32': _f32_attn_case}[build](*args)
+    for args in {'uniform': UNIFORM_CASES, 'f32': F32_ATTN_CASES, 'wgmma_ragged': []}[build]:
+        {'uniform': _uniform_case, 'f32': _f32_attn_case}[build](*args)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -393,7 +385,7 @@ def test_decode_attention(beam, M, pos, n_partials, D):
     case = _dec_case(beam, M, pos, n_partials, D)
     ctx, tk, tv = _run_decode(case)
     _check_decode(case, ctx, tk, tv, 'decode beam=%d M=%d pos=%d np=%d D=%d' % (beam, M, pos, n_partials, D))
-    for grid in (1, 7):      # one CTA walking every item (kPipe look-ahead past kPre), several items per CTA
+    for grid in (1, 7):      # one CTA walking every item (the beam-1 look-ahead past kPre), several items per CTA
         assert torch.equal(_run_decode(case, grid)[0].view(torch.int16), ctx.view(torch.int16)), grid
 
 
@@ -433,7 +425,7 @@ def test_ragged_decode_attention_f32(beam):
     assert torch.equal(_run_decode(_ragged_case(beam, fp32=True, pad=0.0))[0].view(torch.int16), ctx.view(torch.int16))
 
 
-def _run_attention(qkv, B, S, H, lens=None, fp32=False, out=None, q_bs=None, o_bs=None, legacy=False):
+def _run_attention(qkv, B, S, H, lens=None, fp32=False, out=None, legacy=False):
     """gitb200_op_attention(_ex) on q | k | v rows of 3 * H * 64 elements; out defaults to [B, S, d] (bf16; split rows
     [B, S, 3d] in parity mode)."""
     L = _lib()
@@ -442,8 +434,7 @@ def _run_attention(qkv, B, S, H, lens=None, fp32=False, out=None, q_bs=None, o_b
     if out is None:
         out = torch.zeros(B, S, 3 * d if fp32 else d, dtype=torch.bfloat16)
     out = out.cuda()
-    q_bs = S * 3 * d if q_bs is None else q_bs
-    o_bs = S * out.shape[-1] if o_bs is None else o_bs
+    q_bs, o_bs = S * 3 * d, S * out.shape[-1]
     es = qkv.element_size()
     base = qkv.data_ptr()
     args = (base, base + d * es, base + 2 * d * es, out.data_ptr(), B, S, H, 3 * d, 3 * d, q_bs, q_bs, d, o_bs)
@@ -490,22 +481,6 @@ def test_flash_wgmma_uniform_stays_in_bounds(B, S, H):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('S,nw', STRIDED_S)
-def test_flash_mma_strided(S, nw):
-    """Batches with gap rows between them run flash_attn_kernel<nw>; the output's gap rows keep their sentinel."""
-    B, H, gap = 2, 2, 5
-    d = H * 64
-    case = _strided_case(S, nw)
-    g = torch.Generator().manual_seed(14)
-    qkv = torch.randn(B, S + gap, 3 * d, generator=g).bfloat16()
-    qkv[:, :S] = case['qkv']
-    out = torch.full((B, S + gap, d), SENTINEL, dtype=torch.bfloat16)
-    out = _run_attention(qkv, B, S, H, out=out, q_bs=(S + gap) * 3 * d, o_bs=(S + gap) * d)
-    assert (out[:, S:] == SENTINEL).all()
-    _check_attention(case, out[:, :S].float(), 'mma.sync S=%d (NW=%d)' % (S, nw))
-
-
-@pytest.mark.gpu
 @pytest.mark.parametrize('B,S,H,lens', F32_ATTN_CASES)
 def test_attn_f32(B, S, H, lens):
     case = _f32_attn_case(B, S, H, lens)
@@ -540,3 +515,5 @@ def test_op_argument_checks():
     assert rc != 0 and 'outside 1 .. 10' in L.last_error(None)
     rc = lib.gitb200_op_attention_ex(p, p, p, p, 1, 20000, 1, 192, 192, 192 * 20000, 192 * 20000, 64, 0, None, 1, st)
     assert rc != 0 and 'shared memory' in L.last_error(None)
+    rc = lib.gitb200_op_attention_ex(p, p, p, p, 2, 10, 1, 192, 192, 1920 + 192, 1920 + 192, 64, 640, None, 0, st)
+    assert rc != 0 and 'back to back' in L.last_error(None)          # gap rows between the batches
