@@ -8,9 +8,9 @@
 //   * one CTA per SM (132 on an H100; cooperative launch), 8 compute warps + 1 producer warp each;
 //   * every byte the step reads from HBM -- the weight tiles a CTA owns in each GEMM phase, the image K/V of its attention
 //     items and the text K/V so far -- flows through a 12 x 16 KB shared-memory ring that the producer warp fills in
-//     program order with TMA (bulk copies of pre-packed weight tiles, 64-key swizzled K | V box pairs), running as far
-//     ahead of the compute warps as the ring allows, across phase boundaries (only the text K/V of the CURRENT layer waits
-//     for that layer's QKV phase);
+//     program order with TMA (bulk copies of pre-packed weight tiles, swizzled K | V boxes of up to 64 keys: only the key
+//     rows attention reads), running as far ahead of the compute warps as the ring allows, across phase boundaries (only
+//     the text K/V of the CURRENT layer waits for that layer's QKV phase);
 //   * phases (QKV | attention | out-proj | LN | fc1 | fc2 | LN per layer, then LM head | selection + embedding) are
 //     separated by a grid barrier (one release-add + acquire-spin on a global counter -- the cheapest of
 //     the variants tools/barrier_bench.cu times); what crosses a barrier is only the <= 64-row activations, read straight
@@ -38,7 +38,8 @@ constexpr int kMegaThreads = (kMegaComputeWarps + 1) * 32;
 constexpr int kMegaSlots = 12;
 constexpr int kMegaSlotBytes = 16384;
 constexpr int kMegaTileBytes = 12288;      // 8 output features x 768 k x bf16, in mma-fragment order (pack_tiles_kernel)
-constexpr int kMegaKvRows = 64;            // keys per attention chunk: one ring slot = K box (8 KB) | V box (8 KB)
+constexpr int kMegaKvRows = 64;            // keys per attention chunk: one ring slot = K half (8 KB) | V half (8 KB)
+constexpr int kMegaKvSubRows = 16;         // a chunk of fewer keys is fetched in 16-row sub-boxes (2 KB of K, 2 KB of V each)
 constexpr int kMegaMaxRows = 64;
 constexpr int kMegaD = 768, kMegaF = 3072, kMegaH = 12;
 constexpr int kMegaAttItems = 6;           // (sequence, head) attention items of the busiest CTA: ceil(64 * 12 / 132)
@@ -341,7 +342,8 @@ __device__ __forceinline__ float2 ldcg_f2(const float* p) { return __ldcg(reinte
 
 // ---- the kernel ----------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kMegaThreads, 1)
-decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant__ CUtensorMap tmTXT, const MegaParams p) {
+decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant__ CUtensorMap tmTXT,
+                   const __grid_constant__ CUtensorMap tmKV16, const __grid_constant__ CUtensorMap tmTXT16, const MegaParams p) {
   extern __shared__ __align__(1024) uint8_t mega_smem_raw[];
   uint8_t* smem = mega_smem_raw + ((1024u - (smem_u32(mega_smem_raw) & 1023u)) & 1023u);
   uint8_t* ring = smem;                                                  // 12 x 16 KB
@@ -364,7 +366,10 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
   const int R = p.R, M = p.M;
   const int pos = st->pos, step = st->step, cur_len = st->cur_len;
   const int n_kv = (M + kMegaKvRows - 1) / kMegaKvRows;
-  const int n_txt = pos / 64 + 1;               // 64-position boxes of the text K/V cache holding positions 0 .. pos
+  const int n_txt = pos / 64 + 1;               // 64-position chunks of the text K/V cache holding positions 0 .. pos
+  // valid keys of attention round r (image chunks 0 .. n_kv - 1, then text chunks): 64 except in the last image chunk and
+  // the last text chunk.  Producer and consumers both derive it from M and pos, so they agree on which rows are fetched.
+  auto round_keys = [&](int r) { return min(kMegaKvRows, r < n_kv ? M - r * kMegaKvRows : pos + 1 - (r - n_kv) * 64); };
   const int n_items = R * kMegaH;
   const int my_cta_rev = G - 1 - cta;           // attention items are dealt from the last CTA down (those own fewer weights)
   const int n_my_items = (n_items > my_cta_rev) ? (n_items - my_cta_rev + G - 1) / G : 0;
@@ -380,6 +385,8 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
   if (tid == 0) {
     tma_prefetch_desc(&tmKV);
     tma_prefetch_desc(&tmTXT);
+    tma_prefetch_desc(&tmKV16);
+    tma_prefetch_desc(&tmTXT16);
     for (int s = 0; s < kMegaSlots; ++s) {
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], kMegaComputeWarps);
@@ -410,20 +417,39 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
         bulk_load_1d(dst, src, kMegaTileBytes, &full[i % kMegaSlots]);
         publish();
       };
-      // one attention chunk: 64 keys of one (sequence, head): K box at the slot's start, V box 8 KB in
-      auto kv_pair = [&](const CUtensorMap* tm, int row_k, int row_v, int col) {
+      // one attention chunk: up to 64 keys of one (sequence, head) with n valid, K rows at the slot's start, V rows 8 KB
+      // in.  n = 64: one 64-row box each.  n < 64: ceil(n / 16) 16-row boxes each, sub-box s at byte 2048 s of its half --
+      // the rows past the last sub-box are never fetched and never read (keys64 stops at the same 16-key step).  The 128B
+      // swizzle (PTX ISA, tensor copy swizzling modes) XORs the 16-byte chunk index of a row with address bits 7..9, the
+      // row's index within its 1024-byte block; both halves start 1024-byte aligned, so row j of a sub-box at 2048 s lands
+      // at 2048 s + 128 j with chunk c at c ^ (j & 7) -- where row 16 s + j of a 64-row box would ((16 s + j) & 7 == j & 7),
+      // and keys64's ldmatrix addressing serves both.  expect_tx counts the bytes requested (rows past the tensor's end
+      // are zero-filled and still counted).
+      auto kv_pair = [&](const CUtensorMap* tm, const CUtensorMap* tm16, int row_k, int row_v, int col, int n) {
         uint8_t* dst = slot_ready();
-        mbar_arrive_expect_tx(&full[i % kMegaSlots], kMegaSlotBytes);
-        tma_load_2d(dst, tm, &full[i % kMegaSlots], col, row_k);
-        tma_load_2d(dst + 8192, tm, &full[i % kMegaSlots], col, row_v);
+        uint64_t* bar = &full[i % kMegaSlots];
+        if (n >= kMegaKvRows) {
+          mbar_arrive_expect_tx(bar, kMegaSlotBytes);
+          tma_load_2d(dst, tm, bar, col, row_k);
+          tma_load_2d(dst + 8192, tm, bar, col, row_v);
+        } else {
+          const int ns = (n + kMegaKvSubRows - 1) / kMegaKvSubRows;
+          mbar_arrive_expect_tx(bar, ns * 2 * (kMegaKvSubRows * 128));
+          for (int s = 0; s < ns; ++s) {
+            tma_load_2d(dst + s * (kMegaKvSubRows * 128), tm16, bar, col, row_k + s * kMegaKvSubRows);
+            tma_load_2d(dst + 8192 + s * (kMegaKvSubRows * 128), tm16, bar, col, row_v + s * kMegaKvSubRows);
+          }
+        }
         publish();
       };
       for (int l = 0; l < p.n_layers; ++l) {
         const MegaLayer& L = p.layer[l];
         for (int j = 0; j < qkv_n; ++j) tile(L.wqkv + static_cast<size_t>(qkv_t0 + j) * kMegaTileBytes);
         // attention chunks ("units") of this CTA's items, round-major: unit u = r * n_my_items + k is keys 64r .. 64r + 63 of
-        // item k (image keys first, then the text rounds); the consumer deals the units to its 8 warps round-robin
+        // item k (image keys first, then the text rounds), of which round_keys(r) are fetched; the consumer deals the
+        // units to its 8 warps round-robin
         for (int r = 0; r < n_kv + n_txt; ++r) {
+          const int n_keys = round_keys(r);
           if (r == n_kv) {
             // the text K/V of position `pos` exist once every CTA has passed barrier 7l + 1 (after this layer's QKV phase)
             const unsigned int target = static_cast<unsigned int>(G) * (7u * l + 1u);
@@ -440,9 +466,11 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
             const int item = my_cta_rev + kk * G;
             const int b = item / kMegaH, h = item - b * kMegaH;
             if (r < n_kv)
-              kv_pair(&tmKV, (l * 2 + 0) * R * M + b * M + r * kMegaKvRows, (l * 2 + 1) * R * M + b * M + r * kMegaKvRows, h * 64);
+              kv_pair(&tmKV, &tmKV16, (l * 2 + 0) * R * M + b * M + r * kMegaKvRows, (l * 2 + 1) * R * M + b * M + r * kMegaKvRows,
+                      h * 64, n_keys);
             else
-              kv_pair(&tmTXT, ((l * 2 + 0) * R + b) * p.T_alloc + (r - n_kv) * 64, ((l * 2 + 1) * R + b) * p.T_alloc + (r - n_kv) * 64, h * 64);
+              kv_pair(&tmTXT, &tmTXT16, ((l * 2 + 0) * R + b) * p.T_alloc + (r - n_kv) * 64,
+                      ((l * 2 + 1) * R + b) * p.T_alloc + (r - n_kv) * 64, h * 64, n_keys);
           }
         }
         if (cta < 96) tile(L.wo + static_cast<size_t>(cta) * kMegaTileBytes);
@@ -530,7 +558,7 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
     // O += P V run on mma.sync with a 16-row q tile whose row 0 is the query (rows 1..15 zero).  At the end warp k merges
     // the 8 states of item k in warp order (bit-reproducible).  Two block-level barriers per phase, none per unit.
     {
-      const int rounds = n_kv + n_txt;                      // ring chunks per item (64 keys each)
+      const int rounds = n_kv + n_txt;                      // ring chunks per item (up to 64 keys each)
       const uint32_t att_base = rg.idx;
       const int U = n_my_items * rounds;
       uint8_t* qw = q_s + warp * 2048;
@@ -578,13 +606,22 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
 #pragma unroll
           for (int j = 0; j < 8; ++j) { o[j][0] = sl[8 * j + 2 * t]; o[j][1] = sl[8 * j + 2 * t + 1]; }
         }
-        // 64 keys: rows [row0, row0 + 64) of a K box at sK and of a V box at sV; key index = key0 + row, valid below key_end
-        auto keys64 = [&](uint32_t sK, uint32_t sV, int row0, int key0, int key_end) {
+        // up to 64 keys: rows [0, 16 ns) of the K half at sK and the V half at sV -- the ns 16-key steps kv_pair fetched
+        // (ns = 4 for a whole chunk); key index = key0 + row, valid below key_end.  Rows past 16 ns were not fetched and
+        // are not read: their 8-key score groups are skipped (left at 0, then set to -inf by the key_end mask, since
+        // key0 + 16 ns >= key_end) and so are their p.V steps.  Fetched or not, such a key had score -inf, so p = +0: it
+        // added nothing to l and +-0 to o, and skipping it leaves m, l and o as they were (but for the sign of an o that is
+        // exactly zero).  The loops stay fully unrolled with ns as a predicate, so sc / o keep static register indices;
+        // a whole chunk (ns = 4) takes a copy without the predicates, so that its ldmatrix loads can still be issued ahead
+        // of the MMAs.  The first 16-key step (ns >= 1) is unconditional in both copies.
+        auto keys64 = [&](uint32_t sK, uint32_t sV, int key0, int key_end, int ns, auto whole) {
+          constexpr bool kWhole = decltype(whole)::value;
           float sc[8][4];
 #pragma unroll
           for (int jn = 0; jn < 8; ++jn) {
             sc[jn][0] = sc[jn][1] = sc[jn][2] = sc[jn][3] = 0.f;
-            const int krow = row0 + 8 * jn + (lane & 7);
+            if (!kWhole && jn >= 2 && jn >= 2 * ns) continue;
+            const int krow = 8 * jn + (lane & 7);
 #pragma unroll
             for (int kk2 = 0; kk2 < 2; ++kk2) {
               const int chunk = 4 * kk2 + (lane >> 3);
@@ -613,11 +650,13 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
           for (int j = 0; j < 8; ++j) { o[j][0] *= corr; o[j][1] *= corr; }
 #pragma unroll
           for (int kk = 0; kk < 4; ++kk) {                  // 16 keys per k-step = score tiles 2kk, 2kk + 1
+            if (!kWhole && kk > 0 && kk >= ns) continue;    // step 0 unconditional: l_run * corr + its sum still contracts
+                                                            // to one FFMA, as it did before (bit-identical l)
             const float p0 = ex2_approx((sc[2 * kk][0] - m_use) * kLog2e), p1 = ex2_approx((sc[2 * kk][1] - m_use) * kLog2e);
             const float p2 = ex2_approx((sc[2 * kk + 1][0] - m_use) * kLog2e), p3 = ex2_approx((sc[2 * kk + 1][1] - m_use) * kLog2e);
             l_run += (p0 + p1) + (p2 + p3);
             const uint32_t pa[4] = {pack_bf16(p0, p1), 0u, pack_bf16(p2, p3), 0u};   // rows 8..15 of the q tile do not exist
-            const int vrow = row0 + 16 * kk + ((lane >> 3) & 1) * 8 + (lane & 7);
+            const int vrow = 16 * kk + ((lane >> 3) & 1) * 8 + (lane & 7);
 #pragma unroll
             for (int jj = 0; jj < 4; ++jj) {
               const int chunk = 2 * jj + (lane >> 4);
@@ -630,8 +669,11 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
         };
         const uint32_t ci = att_base + static_cast<uint32_t>(u);
         const uint32_t sK = smem_u32(rg.acquire_at(ci));
-        if (r < n_kv) keys64(sK, sK + 8192, 0, r * kMegaKvRows, M);               // image keys 64r ..
-        else keys64(sK, sK + 8192, 0, (r - n_kv) * 64, pos + 1);                 // text positions 64(r - n_kv) ..
+        const int ns = (round_keys(r) + kMegaKvSubRows - 1) / kMegaKvSubRows;
+        const int key0 = (r < n_kv) ? r * kMegaKvRows : (r - n_kv) * 64;         // image keys 64r .. | text positions 64(r - n_kv) ..
+        const int key_end = (r < n_kv) ? M : pos + 1;
+        if (ns == kMegaKvRows / kMegaKvSubRows) keys64(sK, sK + 8192, key0, key_end, ns, std::true_type());
+        else keys64(sK, sK + 8192, key0, key_end, ns, std::false_type());
         rg.release_at(ci);
         if (g == 0) {
           if (t == 0) sl[64] = m_run;

@@ -1221,8 +1221,8 @@ static int prefill_impl(gitb200_engine* h, int B, int beam, int T_alloc, float* 
   const long long kvb = static_cast<long long>(h->kvb());
   TRY(image_rows_buffers(h));
   {
-    // decode_mega_kernel fetches whole 64-position boxes of the text cache and masks the positions past the caption's end
-    // by giving them probability 0 -- which only works if what lies there is finite: a fresh allocation is zeroed once
+    // decode_mega_kernel fetches the text cache in 16-position steps up to the caption's end and masks the positions past
+    // it in the last step by giving them probability 0 -- which only works if what lies there is finite: a fresh allocation is zeroed once
     // (afterwards the buffer only ever holds K/V values or zeros of one element size).  A parity switch keeps the buffer
     // but changes the element size: fp32 K/V read as bf16 pairs hold Inf / NaN patterns, so the cache is zeroed again.
     const void* before = h->txt_kv.p;
