@@ -5,7 +5,7 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, 'libgitb200.so')
-ABI_VERSION = 9
+ABI_VERSION = 10
 
 c_void_p, c_int, c_int64, c_float, c_char_p = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_char_p
 c_ll = ctypes.c_longlong
@@ -27,6 +27,15 @@ class ImageDesc(ctypes.Structure):
                 ('resize_h', ctypes.c_int32), ('resize_w', ctypes.c_int32), ('crop_top', ctypes.c_int32),
                 ('crop_left', ctypes.c_int32), ('out_h', ctypes.c_int32), ('out_w', ctypes.c_int32),
                 ('dst_offset', ctypes.c_int64)]
+
+
+class GemmDesc(ctypes.Structure):
+    """gitb200_gemm_desc: one launch of the GEMM kernel as its launcher sees it (gitb200_op_gemm_ex)."""
+    _fields_ = ([('a', c_void_p), ('b', c_void_p), ('bias', c_void_p), ('resid', c_void_p), ('out', c_void_p * 3),
+                 ('lse_target', c_void_p), ('skip', c_void_p)] +
+                [(n, ctypes.c_int64) for n in ('lda', 'ldb', 'ld_resid', 'ldo', 'batch_stride', 'split_stride')] +
+                [(n, ctypes.c_int32) for n in ('M', 'N', 'K', 'act', 'out_bf16', 'split3', 'transposed', 'k_splits', 'bn',
+                                               'seg_n', 'rows_per_batch', 'row_offset')])
 
 
 SEARCH_GREEDY, SEARCH_BEAM = 0, 1
@@ -75,6 +84,12 @@ SIGNATURES = {
                                 c_int, c_int, c_int, c_void_p]),
     'gitb200_op_layernorm': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p,
                                      c_int, c_int, c_void_p]),
+    'gitb200_op_gemm_ex': (c_int, [ctypes.POINTER(GemmDesc), ctypes.POINTER(c_int), c_void_p]),
+    'gitb200_op_layernorm_ex': (c_int, [c_void_p, c_int, c_ll, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_void_p,
+                                        c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_int,
+                                        c_void_p]),
+    'gitb200_op_lse_combine': (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_void_p,
+                                       c_void_p, c_void_p, c_void_p, c_void_p]),
     'gitb200_op_attention': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_ll, c_ll, c_ll, c_ll,
                                      c_ll, c_ll, c_void_p]),
     'gitb200_op_attention_ex': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_ll, c_ll, c_ll,

@@ -44,7 +44,7 @@
 using namespace gitb200;
 typedef __nv_bfloat16 bf16;
 
-#define GITB200_ABI_VERSION 9
+#define GITB200_ABI_VERSION 10
 
 // ------------------------------------------------------------------------------------------------
 // errors
@@ -390,15 +390,18 @@ static int pick_bn(const gitb200_engine* h, int M, int N, bool transposed) {
   return N > 192 ? 256 : (N > 128 ? 192 : 128);
 }
 
+// Splits launch_gemm runs for `requested` over K: every split takes ceil(k-blocks / requested) 64-wide k-blocks, and the
+// splits that would be left without one are dropped (8 requested over 12 k-blocks -> 6).
+static int effective_k_splits(int K, int requested) {
+  const int kb_total = (K + 63) / 64;
+  const int splits = std::max(1, std::min(requested, kb_total));
+  const int kb_per = (kb_total + splits - 1) / splits;
+  return (kb_total + kb_per - 1) / kb_per;
+}
+
 static int launch_gemm(gitb200_engine* h, GemmCall c, cudaStream_t st) {
   GemmParams& p = c.p;
-  if (p.k_splits < 1) p.k_splits = 1;
-  const int kb_total = (p.K + 63) / 64;
-  if (p.k_splits > kb_total) p.k_splits = kb_total;
-  {
-    const int kb_per = (kb_total + p.k_splits - 1) / p.k_splits;
-    p.k_splits = (kb_total + kb_per - 1) / kb_per;  // no empty split
-  }
+  p.k_splits = effective_k_splits(p.K, p.k_splits);
   if (p.seg_n <= 0) p.seg_n = p.N;
   if (p.rows_per_batch <= 0) {
     p.rows_per_batch = p.M;

@@ -62,7 +62,8 @@ enum { GITB200_F32 = 0, GITB200_BF16 = 1, GITB200_I64 = 2 };
 int gitb200_create(const gitb200_config* cfg, int device, gitb200_engine** out);
 void gitb200_destroy(gitb200_engine* h);
 const char* gitb200_last_error(const gitb200_engine* h);
-/* ABI version of the library (bumped on any signature change): 9 (gitb200_score, gitb200_op_text_attention). */
+/* ABI version of the library (bumped on any signature change): 10 (gitb200_op_gemm_ex, gitb200_op_layernorm_ex,
+ * gitb200_op_lse_combine); 9 added gitb200_score and gitb200_op_text_attention. */
 int gitb200_abi_version(void);
 
 /* Replaces: torch_common.load_state_dict -> module parameters           torch_common.py:93-145.
@@ -220,6 +221,48 @@ int gitb200_op_gemm(const void* a_dev, const void* w_dev, const float* bias_dev,
 int gitb200_op_layernorm(const float* x_dev, const float* bias_dev, const float* resid_dev, const float* gamma_dev,
                          const float* beta_dev, float eps, float* out_f32_dev, void* out_bf16_dev, int rows, int D,
                          void* stream);
+/* One launch of gemm_bf16_wgmma with everything its launcher takes, in the kernel's own operand terms:
+ *   C[m][n] = sum_k a[m][k] * b[n][k], a [M, K] (128-row tiles) and b [N, K] (bn-row tiles) bf16, row pitches lda / ldb.
+ * transposed == 0: out[seg][row_map(m)][n % seg_n] = C (+bias[n]) (+act) (+resid[m][n]), seg = n / seg_n (up to three column
+ *   segments with their own base pointers and the one row pitch ldo), row_map(m) = (m / rows_per_batch) * batch_stride +
+ *   m % rows_per_batch + row_offset (rows_per_batch <= 0: identity); resid fp32, pitch ld_resid, may be out[0] (in place).
+ *   split3: bf16 rows [hi | lo | hi] of 3 * N columns.  lse_target != NULL: the LM-head statistics epilogue, out[0] =
+ *   float4 (max, sum exp(x - max), sum x, x[target]) per (row, half tile) at [m * ldo + 2 * (n / 256) + half], bias required.
+ * transposed != 0 (swap-AB: a = weight [features, K], b = activations [rows, K]): out[0][n][m] = C (+bias[m]) (+act).
+ *   k_splits > 1: split s leaves its raw fp32 partial sums at out[0] + s * split_stride (nothing adds them up);
+ *   *k_splits_out (may be NULL) receives the number of splits that ran (empty ones are dropped: 8 over 12 k-blocks -> 6).
+ * act: 0 none, 1 QuickGELU (tanh.approx), 2 erf-GELU, 3 QuickGELU (expf).  bn: tile width, 0 = heuristic.
+ * skip: NULL or a device int; non-zero -> the launch stores nothing. */
+typedef struct gitb200_gemm_desc {
+  const void* a;
+  const void* b;
+  const float* bias;
+  const float* resid;
+  void* out[3];
+  const int32_t* lse_target;
+  const int32_t* skip;
+  int64_t lda, ldb, ld_resid, ldo, batch_stride, split_stride;
+  int32_t M, N, K;
+  int32_t act, out_bf16, split3, transposed, k_splits, bn;
+  int32_t seg_n, rows_per_batch, row_offset;
+} gitb200_gemm_desc;
+int gitb200_op_gemm_ex(const gitb200_gemm_desc* desc, int* k_splits_out, void* stream);
+/* gitb200_op_layernorm with the rest of layernorm_kernel's inputs: x_dev is the first of n_partials (>= 1) split-K
+ * partial buffers, partial_stride elements apart, added in split order; split3: out_bf16 rows [hi | lo | hi] (3 * D);
+ * temb_dev [F, D] or NULL with remap_B / F / L (remap_F == 0: none): input row (f * B + b) * L + l -> output row
+ * (b * F + f) * L + l, temb[f] added after the normalisation; skip_flag_dev: NULL or a device int, non-zero -> no-op;
+ * pre != 0: the <768, PRE = true> instantiation of the decode chain (D = 768 only). */
+int gitb200_op_layernorm_ex(const float* x_dev, int n_partials, long long partial_stride, const float* bias_dev,
+                            const float* resid_dev, const float* gamma_dev, const float* beta_dev, float eps,
+                            float* out_f32_dev, void* out_bf16_dev, int rows, int D, int split3, const float* temb_dev,
+                            int remap_B, int remap_F, int remap_L, const int32_t* skip_flag_dev, int pre, void* stream);
+/* lse_combine_kernel, then loss_mean_kernel when loss_dev != NULL, on caller-supplied LM-head partials: parts_dev float4
+ * [rows, n_parts] (max, sum exp, sum x, x[target]), rows = captions * T, targets_dev int32 [rows], need_predict_dev int64
+ * [rows] -> logprob_dev [captions, T - 1], row_loss_dev fp32 [rows], row_valid_dev int32 [rows], loss_dev fp32 [1]
+ * (NaN when no row is valid). */
+int gitb200_op_lse_combine(const void* parts_dev, int n_parts, int rows, int T, int V, const int32_t* targets_dev,
+                           const int64_t* need_predict_dev, float eps, float* logprob_dev, float* row_loss_dev,
+                           int32_t* row_valid_dev, float* loss_dev, void* stream);
 /* Non-causal multi-head attention over packed bf16 rows: q/k/v [B, S, H*64] with the given row strides (elements);
  * batches are stored back to back (q_batch_stride = S * q_row_stride, kv_batch_stride = S * kv_row_stride; other batch
  * strides are refused); out bf16 [B, S, H*64] with its own row and batch strides. softmax(q k^T / 8) v. */

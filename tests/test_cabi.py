@@ -32,6 +32,7 @@ def test_struct_layouts_match_header():
     from generativeimage2text_b200 import _lib
     assert ctypes.sizeof(_lib.Config) == 14 * 4
     assert ctypes.sizeof(_lib.Search) == 5 * 4
+    assert ctypes.sizeof(_lib.GemmDesc) == 9 * 8 + 6 * 8 + 12 * 4    # gitb200_gemm_desc: pointers, int64, int32
 
 
 def test_no_cpu_fallback():

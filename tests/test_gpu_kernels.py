@@ -1,5 +1,6 @@
 """GPU: every hand-written kernel through its C-ABI entry point against a plain PyTorch fp32 statement of
-the same op on the same (bf16-rounded) inputs."""
+the same op on the same (bf16-rounded) inputs.  The GEMM and LayerNorm tests here are a smoke layer: every GEMM
+instantiation, epilogue form and split-K / LM-head consumer is compared with fp64 in tests/test_gpu_gemm.py."""
 import ctypes
 
 import pytest
