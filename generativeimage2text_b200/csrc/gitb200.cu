@@ -158,6 +158,8 @@ struct gitb200_engine {
   DevBuf y_t, qb_t, mega_bar;                               // decode_mega_kernel: pre-LN sums, bf16 q, grid-barrier counters
   DevBuf state, next_token, logprob_sum, tokens_i64, stage_img, stage_tok, stage_lp, prefix_dev;
   DevBuf beam_ws;                                           // beam-search bookkeeping (search.cuh)
+  BeamState beam_s{};                                       // ... as the last beam generate carved it (gitb200_debug_read)
+  int beam_B = 0, beam_max_steps = 0;                       // 0: the last prefill was not a beam generate
   DevBuf sc_t, sc_x, sc_h, sc_q, sc_kv, sc_ctx, sc_u;       // caption scoring: text-row workspaces (score_impl)
   DevBuf sc_tgt, sc_part, sc_loss, sc_valid, sc_index;      // ... LM-head targets / statistics, per-row losses, op image_index
   DevBuf sel_ws;                                            // greedy selection partials

@@ -12,6 +12,11 @@
 //   beam_finalize_kernel : decoded[B, max_steps] (EOS padded) and the length-normalised score.
 // The text KV cache is never copied: src_row[r][j] names the physical row that holds position j of
 // logical row r's history.
+//
+// Candidate order: (score desc, beam asc, logit desc, token asc).  A row's list is ranked on the raw logit (lower token on
+// exact ties); the score ((z - max) - log_sum) + beam_score is increasing in z in exact arithmetic, but fp32 can round two
+// different logits of one row to the same score (e.g. z - max = -100 for a logit one ulp apart), and those keep the logit
+// order -- the order of their exact scores.  The merge breaks equal scores of different beams by the lower flat index.
 #pragma once
 #include "ptx.cuh"
 #include "rowops.cuh"

@@ -338,7 +338,17 @@ int gitb200_preproc_coeffs(int in_size, int out_size, int32_t* ksize_out, int32_
 /* Debug: copies one decode-step work buffer of the engine ("x", "y" fp32 [rows,768]; "hb", "ctx", "qb" bf16 [rows,768];
  * "ub" bf16 [rows,3072]) or cache ("img_kv": the image K/V [layer][k|v][image][token][768] of the last prefill, batch x
  * tokens rows; "txt_kv": the text K/V [layer][k|v][row][T_alloc][768], T_alloc = bytes / (layers * 2 * rows * 768 * element
- * size); both bf16, fp32 in parity mode) to host memory after a device synchronise.  Returns bytes copied or -1. */
+ * size); both bf16, fp32 in parity mode) to host memory after a device synchronise.  Beam search bookkeeping, current
+ * side of each ping-pong:
+ *   "src_row"     int32 [rows][T_alloc]: the text-K/V indirection table the next beam step reads (position j of logical
+ *                 row r is held by physical row src_row[r][j]); after a beam generate or the raw decode_step API;
+ *   "beam_ids"    int64 [rows][max_steps]: the token history (input_ids) of each beam, after a beam generate;
+ *   "beam_scores" fp32 [rows]: the running beam scores, after a beam generate;
+ *   "beam_hyp"    [4][batch] 4-byte words, after a beam generate: done (int32), hyp_len (int32, 0 = no hypothesis),
+ *                 hyp_score (fp32, length-normalised), worst_score (fp32).
+ *   "beam_cand"   [2][rows][8] 4-byte words, after a beam generate: the last step's per-row candidate list, scores
+ *                 (fp32: log-softmax + beam score) then token ids (int32); the first 2 * beam entries of a row are valid.
+ * Returns bytes copied or -1. */
 long long gitb200_debug_read(gitb200_engine* h, const char* name, void* out_host, long long max_bytes);
 /* Debug aid: in-situ timeline of the decode-step kernels. enable != 0 arms it; enable == 0 copies up to
  * max_entries (globaltimer ns, kernel id) pairs to out_host, disarms, and returns the number of entries. */

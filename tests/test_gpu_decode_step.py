@@ -20,18 +20,12 @@ parity-mode -> default-mode sequence on one engine.
 """
 import contextlib
 import ctypes
-import math
 
 import pytest
 import torch
 
 import git_oracle
-
-V = 30522
-D = 768
-H = 12
-EOS = 102
-CLS = 101
+from decode_ref import V, D, EOS, CLS, bf16, RefWeights, ref_step, expected_selection
 
 # Largest |engine - ref_step| per path and compared quantity: about 2x the largest error observed over these cases on an
 # H100 80GB HBM3 (132 SMs, 700 W power limit), given after each.  The bf16 quantities differ from the reference by whole
@@ -75,131 +69,6 @@ def _report_measured_errors():
 
 class Tok:
     cls_token_id, sep_token_id = CLS, EOS
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# fp64 reference of one greedy decode step
-# ---------------------------------------------------------------------------------------------------------------------
-def bf16(t):
-    """Round to bfloat16 (to nearest, ties to even, from the fp32 value) and return it as fp64."""
-    x = t.to(torch.float32).contiguous()
-    b = x.view(torch.int32).to(torch.int64) & 0xFFFFFFFF
-    b = (b + 0x7FFF + ((b >> 16) & 1)) & 0xFFFF0000
-    b = torch.where(b >= 2 ** 31, b - 2 ** 32, b)
-    return b.to(torch.int32).view(torch.float32).to(torch.float64)
-
-
-def _ln(x, g, b, eps):
-    mu = x.mean(-1, keepdim=True)
-    var = ((x - mu) ** 2).mean(-1, keepdim=True)
-    return (x - mu) / torch.sqrt(var + eps) * g + b
-
-
-def _gelu_erf(x):
-    return x * 0.5 * (1.0 + torch.erf(x / math.sqrt(2.0)))
-
-
-class RefWeights(object):
-    """The decoder's weights in fp64; GEMM weights and the tied LM-head matrix rounded to bf16 when `rounding`."""
-
-    def __init__(self, sd, rounding=True):
-        w = (lambda k: bf16(sd[k])) if rounding else (lambda k: sd[k].double())
-        f = lambda k: sd[k].double()
-        t = 'textual.'
-        self.rounding = rounding
-        self.words = f(t + 'embedding.words.weight')
-        self.lm = bf16(self.words) if rounding else self.words
-        self.positions = f(t + 'embedding.positions.weight')
-        self.lne = (f(t + 'embedding.layer_norm.weight'), f(t + 'embedding.layer_norm.bias'))
-        self.out_bias = f(t + 'output.bias')
-        self.layers = []
-        for j in range(6):
-            b = t + 'transformer.encoder.layer.%d.' % j
-            a = b + 'attention.'
-            self.layers.append(dict(
-                wq=w(a + 'self.query.weight'), bq=f(a + 'self.query.bias'),
-                wk=w(a + 'self.key.weight'), bk=f(a + 'self.key.bias'),
-                wv=w(a + 'self.value.weight'), bv=f(a + 'self.value.bias'),
-                wo=w(a + 'output.dense.weight'), bo=f(a + 'output.dense.bias'),
-                ln1=(f(a + 'output.LayerNorm.weight'), f(a + 'output.LayerNorm.bias')),
-                w1=w(b + 'intermediate.dense.weight'), b1=f(b + 'intermediate.dense.bias'),
-                w2=w(b + 'output.dense.weight'), b2=f(b + 'output.dense.bias'),
-                ln2=(f(b + 'output.LayerNorm.weight'), f(b + 'output.LayerNorm.bias'))))
-
-    def embed(self, tokens, pos):
-        """LN(words[token] + positions[pos], eps 1e-8) in fp64 (reference layers/decoder.py:65-78)."""
-        return _ln(self.words[tokens] + self.positions[pos], self.lne[0], self.lne[1], 1e-8)
-
-
-def ref_step(W, img_k, img_v, txt_k, txt_v, tokens, pos, n_layers=6, q_bf16=True, defect=None):
-    """One greedy decode step of R rows at text position `pos`.
-
-    img_k / img_v: per layer [R, M, 768] (the image K/V cache); txt_k / txt_v: per layer [R, pos, 768] (text positions
-    0 .. pos - 1); tokens: int64 [R], the token fed at `pos`.  q_bf16: the path stores q / 8 as bf16 (the persistent kernel;
-    the chain keeps it in fp32).  defect: None or (kind, index[, layer]) -- one planted error in that layer (default: the
-    last layer run)
-    ('wo' | 'w1' | 'fc2' tile, 'fc2' as (tile, k slice)), in the LM head ('lm' tile), or in its attention ('chunk': a 64-key
-    image chunk, 'img_last': key M - 1, 'newest': the text key at pos, all masked out).
-    Returns {'layers': [per layer: qb, k, v, ctx, y, xa, ub, x], 'logits': [R, V]}."""
-    bf = bf16 if W.rounding else (lambda t: t.double())
-    kind, idx = defect[:2] if defect is not None else (None, None)
-    at = (defect[2] if defect is not None and len(defect) > 2 else n_layers - 1)
-    R = tokens.shape[0]
-    x = W.embed(tokens, pos)
-    out = {'layers': []}
-    for j in range(n_layers):
-        L = W.layers[j]
-        last = j == at
-        hb = bf(x)
-        q = hb @ L['wq'].T + L['bq']
-        qb = bf(q / 8.0) if (q_bf16 and W.rounding) else q / 8.0
-        k = bf(hb @ L['wk'].T + L['bk'])
-        v = bf(hb @ L['wv'].T + L['bv'])
-        ik, iv = img_k[j].double(), img_v[j].double()
-        M = ik.shape[1]
-        K = torch.cat([ik, txt_k[j].double(), k[:, None]], dim=1)
-        Vv = torch.cat([iv, txt_v[j].double(), v[:, None]], dim=1)
-        S = K.shape[1]
-        s = torch.einsum('rhd,rshd->rhs', qb.reshape(R, H, 64), K.reshape(R, S, H, 64))
-        if last and kind in ('chunk', 'img_last', 'newest'):
-            drop = {'chunk': slice(64 * idx, min(64 * idx + 64, M)), 'img_last': slice(M - 1, M),
-                    'newest': slice(S - 1, S)}[kind]
-            s[:, :, drop] = float('-inf')
-        p = torch.softmax(s, dim=-1)
-        ctx = bf(torch.einsum('rhs,rshd->rhd', p, Vv.reshape(R, S, H, 64)).reshape(R, D))
-        wo, w1, w2 = L['wo'], L['w1'], L['w2']
-        if last and kind == 'wo':
-            wo = wo.clone()
-            wo[8 * idx:8 * idx + 8] = 0
-        if last and kind == 'w1':
-            w1 = w1.clone()
-            w1[8 * idx:8 * idx + 8] = 0
-        if last and kind == 'fc2':
-            w2 = w2.clone()
-            w2[8 * idx[0]:8 * idx[0] + 8, 768 * idx[1]:768 * idx[1] + 768] = 0
-        y = x + (ctx @ wo.T + L['bo'])
-        xa = _ln(y, L['ln1'][0], L['ln1'][1], 1e-12)
-        ub = bf(_gelu_erf(bf(xa) @ w1.T + L['b1']))
-        x = _ln(xa + (ub @ w2.T + L['b2']), L['ln2'][0], L['ln2'][1], 1e-12)
-        out['layers'].append(dict(qb=qb, k=k, v=v, ctx=ctx, y=y, xa=xa, ub=ub, x=x))
-    logits = bf(x) @ W.lm.T + W.out_bias
-    if kind == 'lm':
-        logits[:, 8 * idx:8 * idx + 8] = W.out_bias[8 * idx:8 * idx + 8]
-    out['logits'] = logits
-    return out
-
-
-def expected_selection(z, tokens_in, first):
-    """Greedy choice and its log-prob from raw step logits z [R, V] (fp32 as dumped): the no-repeat mask (-10000 at the
-    token fed, reference layers/decoder.py:330) where first[r] is False, arg-max with the lowest index on ties, fp64
-    log-softmax."""
-    z = z.double().clone()
-    for r in range(z.shape[0]):
-        if not first[r]:
-            z[r, int(tokens_in[r])] = -10000.0
-    tok = torch.argmax(z, dim=1)           # the first maximal index
-    lp = torch.log_softmax(z, dim=1).gather(1, tok[:, None])[:, 0]
-    return tok, lp
 
 
 # ---------------------------------------------------------------------------------------------------------------------
