@@ -106,6 +106,13 @@ struct TmapKey {
   }
 };
 
+// Geometry of decode_attn_kernel (dec_attn_geometry).
+struct DecAttnGeom {
+  int chunk_rows, box_rows;   // DecAttnParams::chunk_rows / box_rows
+  size_t smem;                // dynamic shared memory per CTA
+  int grid;                   // CTAs the engine launches
+};
+
 struct gitb200_engine {
   gitb200_config cfg;
   int device = 0;
@@ -114,13 +121,11 @@ struct gitb200_engine {
   int64_t launches = 0;
   bool use_graph = true;
   bool use_pdl = true;
-  bool use_chain = true;
   // fp32-grade parity mode: every GEMM operand is a (hi, lo) bf16 pair and each GEMM computes a_hi w_hi + a_lo w_hi +
   // a_hi w_lo in ONE pass of the same wgmma kernel (activations stored [hi | lo | hi], weights [hi | hi | lo] along K);
   // attention, K/V caches and q/k/v stay fp32; exact QuickGELU.  ~3x the GEMM work: a verification mode (the north star's
   // "logits within 1e-3" against the fp32 reference), not a serving mode.  Weights must be (re-)uploaded after switching.
   bool use_mega = true;   // greedy decode steps of <= 64 sequences through the persistent decode_mega_kernel
-  bool mega_coop = true;  // ... launched cooperatively (co-residency of its one-per-SM CTAs guaranteed by the driver)
   bool mega_ready = false;
   int debug_layers = -1;  // debugging: run only the first n decoder layers in the decode step (both step paths); -1 = all
   bool parity = false;
@@ -151,7 +156,7 @@ struct gitb200_engine {
 
   // workspaces
   DevBuf x, h, qkv, ctx, u, feats, feats_f32, pos_interp;   // encoder
-  DevBuf pt, pxd, phd, pq, pctx, pu;                        // prefill
+  DevBuf pt, pxd, phd, pq, pctx, pu;                        // decoder-layer pass (image rows, caption rows)
   DevBuf img_kv, txt_kv, src_row[2];                        // caches
   size_t txt_kv_eb = 0;                                     // element size (kvb()) the text cache was last zeroed for
   DevBuf xd_t, hd_t, qkv_t, ctx_t, t_t, u_t, logits;        // decode step
@@ -160,12 +165,11 @@ struct gitb200_engine {
   DevBuf beam_ws;                                           // beam-search bookkeeping (search.cuh)
   BeamState beam_s{};                                       // ... as the last beam generate carved it (gitb200_debug_read)
   int beam_B = 0, beam_max_steps = 0;                       // 0: the last prefill was not a beam generate
-  DevBuf sc_t, sc_x, sc_h, sc_q, sc_kv, sc_ctx, sc_u;       // caption scoring: text-row workspaces (score_impl)
-  DevBuf sc_tgt, sc_part, sc_loss, sc_valid, sc_index;      // ... LM-head targets / statistics, per-row losses, op image_index
+  DevBuf sc_kv, sc_tgt, sc_part, sc_loss, sc_valid, sc_index;   // caption scoring: one layer's text K/V, LM-head targets /
+                                                               // statistics, per-row losses, op image_index
   DevBuf sel_ws;                                            // greedy selection partials
   DevBuf chain;                                             // decode-step kernel chain completion counters [64]
-  int attn_chunk_rows = 0, attn_box_rows = 0, attn_grid = 0;
-  size_t attn_smem = 0;
+  DecAttnGeom attn_geom{};                                  // decode_attn_kernel geometry of the last prefill
   int cur_B = 0, cur_frames = 0, cur_M = 0, cur_beam = 1, T_alloc = 0, cur_rows = 0, cur_src = 0;
 
   EncodeTiledFn encode_tiled = nullptr;
@@ -202,15 +206,6 @@ struct gitb200_engine {
   float sample_temperature = 1.0f;
   bool constrained = false;            // this call's greedy selection runs constrained_select_kernel
   int64_t* pend_tok_host = nullptr;  // host-buffer variant: results land here
-};
-
-// Row range of one decode chain (the whole batch; kept as a struct so that step_layers reports its chain tail).
-struct Lane {
-  int row0 = 0, rows = 0;   // sequences (images * beam)
-  int b0 = 0, nb = 0;       // images
-  cudaStream_t st = nullptr;
-  int chain_idx = 0;        // out: chain position / CTAs of the last kernel launched by step_layers
-  unsigned int chain_ctas = 0;
 };
 
 static void drop_step_graphs(gitb200_engine* h) {
@@ -436,6 +431,25 @@ static GemmCall gemm_plain(const bf16* A, long long lda, const bf16* W, long lon
   c.p.seg_n = N;
   return c;
 }
+// Output of a row-pass GEMM (encoder, decoder-layer pass, LM heads) in the engine's precision mode:
+//   F32      fp32 [M, N] (+ resid, which may alias out);
+//   OPERAND  the A operand of the next GEMM: bf16 [M, N], or [hi | lo | hi] rows of 3 N columns in parity mode;
+//   QKV      attention inputs: bf16, or fp32 in parity mode.
+enum class RowOut { F32, OPERAND, QKV };
+// gemm_plain over the logical reduction length K: parity mode stores every operand at 3 K (activations [hi | lo | hi],
+// weights [hi | hi | lo]) and computes QuickGELU exactly.
+static GemmCall gemm_rows(const gitb200_engine* h, RowOut kind, const bf16* A, const bf16* W, int M, int N, int K,
+                          const float* bias, int act, const float* resid, void* out) {
+  const int ks = h->ks();
+  const bool bf16_out = kind == RowOut::OPERAND || (kind == RowOut::QKV && !h->parity);
+  GemmCall c = gemm_plain(A, static_cast<long long>(K) * ks, W, static_cast<long long>(K) * ks, M, N, K * ks, bias,
+                          (h->parity && act == ACT_QUICKGELU) ? ACT_QUICKGELU_EXACT : act, resid, out, bf16_out);
+  if (kind == RowOut::OPERAND && h->parity) {
+    c.p.split3 = 1;
+    c.p.ldo = 3LL * N;
+  }
+  return c;
+}
 // Skinny decode-step GEMM: out[r][f] = sum_k X[r][k] W[f][k] (+bias[f]) (+act) -- swap-AB, transposed epilogue.
 // k_splits > 1: split s writes its partial sums to out + s * rows * ldo (fp32); the consumer adds them in split order.
 static GemmCall gemm_skinny(const bf16* X, long long ldx, const bf16* W, long long ldw, int rows, int feats, int K,
@@ -472,6 +486,13 @@ static LnParams ln_params(const float* x, const float* bias, const float* resid,
   p.out_f32 = of32; p.out_bf16 = obf16; p.rows = rows;
   return p;
 }
+// ln_params whose bf16 output is the next GEMM's A operand: [hi | lo | hi] rows in parity mode.
+static LnParams ln_operand(const gitb200_engine* h, const float* x, const float* g, const float* b, float eps, float* of32,
+                           bf16* obf16, int rows) {
+  LnParams p = ln_params(x, nullptr, nullptr, g, b, eps, of32, obf16, rows);
+  p.split3 = h->parity ? 1 : 0;
+  return p;
+}
 
 // Raises `kernel`'s dynamic shared-memory limit to smem bytes on the engine's device; the attribute is set once per kernel,
 // device and larger size (the parity and decode attention kernels size their shared memory per call).
@@ -487,62 +508,100 @@ static int set_dyn_smem(gitb200_engine* h, const void* kernel, size_t smem) {
   return 0;
 }
 
-// Non-causal attention (attention.cuh: flash_attn_wgmma_kernel) for batches stored back to back (row b * S + i of the
-// q / k / v views), which is every ViT and prefill call; TMA needs the row pitch and the bases 16-byte aligned (get_tmap
-// checks).
-static int launch_attention(gitb200_engine* h, const AttnParams& ap, cudaStream_t st) {
-  if (ap.q_bs != static_cast<long long>(ap.S) * ap.q_rs || ap.kv_bs != static_cast<long long>(ap.S) * ap.kv_rs)
+// Self attention (attention.cuh): non-causal, B batches of S rows.  q / k / v rows q_rs / kv_rs elements apart and batches
+// q_bs / kv_bs apart; out rows o_rs apart and batches o_bs apart.  bf16: flash_attn_wgmma_kernel, which reads whole
+// batches by TMA (batches back to back, 16-byte aligned bases and pitches: get_tmap checks).  fp32 (parity mode):
+// attn_f32_kernel, fp32 q / k / v and out rows in the [hi | lo | hi] format of 3 * H * 64 columns.
+struct SelfAttn {
+  const void* q;
+  const void* k;
+  const void* v;
+  bf16* out;
+  int B, S, H;
+  long long q_rs, kv_rs, q_bs, kv_bs, o_rs, o_bs;
+  const int* seq_lens;   // null, or [B] valid rows of each batch
+};
+static int launch_self_attention(gitb200_engine* h, const SelfAttn& a, bool fp32, cudaStream_t st) {
+  if (fp32) {
+    AttnF32Params p{};
+    p.q = static_cast<const float*>(a.q); p.k = static_cast<const float*>(a.k); p.v = static_cast<const float*>(a.v);
+    p.out = a.out;
+    p.B = a.B; p.S = a.S; p.H = a.H; p.d_model = a.H * 64;
+    p.q_rs = a.q_rs; p.kv_rs = a.kv_rs; p.q_bs = a.q_bs; p.kv_bs = a.kv_bs; p.o_bs = a.o_bs;
+    p.seq_lens = a.seq_lens;
+    const size_t smem = static_cast<size_t>(4) * (64 + p.S) * sizeof(float);
+    if (smem > 200 * 1024) return fail(h, "parity attention: %d keys do not fit in shared memory", p.S);
+    TRY(set_dyn_smem(h, reinterpret_cast<const void*>(attn_f32_kernel), smem));
+    const long long items = static_cast<long long>(p.B) * p.H * p.S;
+    attn_f32_kernel<<<static_cast<unsigned int>((items + 3) / 4), 128, smem, st>>>(p);
+    CKL(h, "attn_f32_kernel");
+    return 0;
+  }
+  if (a.q_bs != static_cast<long long>(a.S) * a.q_rs || a.kv_bs != static_cast<long long>(a.S) * a.kv_rs)
     return fail(h, "attention: batches must be stored back to back (batch stride = S * row stride)");
-  AttnParams p = ap;
+  AttnParams p{};
+  p.q = static_cast<const bf16*>(a.q); p.k = static_cast<const bf16*>(a.k); p.v = static_cast<const bf16*>(a.v);
+  p.out = a.out;
+  p.B = a.B; p.S = a.S; p.H = a.H;
+  p.q_rs = a.q_rs; p.kv_rs = a.kv_rs; p.q_bs = a.q_bs; p.kv_bs = a.kv_bs; p.o_rs = a.o_rs; p.o_bs = a.o_bs;
   p.scale_log2 = 0.125f * 1.44269504088896340736f;
-  const long long rows = static_cast<long long>(ap.B) * ap.S;
+  p.seq_lens = a.seq_lens;
+  const long long rows = static_cast<long long>(a.B) * a.S;
   CUtensorMap tq, tk, tv;
-  TRY(get_tmap(h, ap.q, rows, ap.H * 64, ap.q_rs, kAttnWgRows, &tq));
-  TRY(get_tmap(h, ap.k, rows, ap.H * 64, ap.kv_rs, kAttnWgRows, &tk));
-  TRY(get_tmap(h, ap.v, rows, ap.H * 64, ap.kv_rs, kAttnWgRows, &tv));
-  const dim3 grid((ap.S + kAttnWgRows - 1) / kAttnWgRows, ap.H, ap.B);
-  if (ap.seq_lens != nullptr) flash_attn_wgmma_kernel<true><<<grid, 128, kAttnWgSmem, st>>>(tq, tk, tv, p);
+  TRY(get_tmap(h, a.q, rows, a.H * 64, a.q_rs, kAttnWgRows, &tq));
+  TRY(get_tmap(h, a.k, rows, a.H * 64, a.kv_rs, kAttnWgRows, &tk));
+  TRY(get_tmap(h, a.v, rows, a.H * 64, a.kv_rs, kAttnWgRows, &tv));
+  const dim3 grid((a.S + kAttnWgRows - 1) / kAttnWgRows, a.H, a.B);
+  if (a.seq_lens != nullptr) flash_attn_wgmma_kernel<true><<<grid, 128, kAttnWgSmem, st>>>(tq, tk, tv, p);
   else flash_attn_wgmma_kernel<false><<<grid, 128, kAttnWgSmem, st>>>(tq, tk, tv, p);
   CKL(h, "flash_attn_wgmma_kernel");
   return 0;
 }
 
-static int launch_attention_f32(gitb200_engine* h, const AttnF32Params& p, cudaStream_t st) {
-  const size_t smem = static_cast<size_t>(4) * (64 + p.S) * sizeof(float);
-  if (smem > 200 * 1024) return fail(h, "parity attention: %d keys do not fit in shared memory", p.S);
-  TRY(set_dyn_smem(h, reinterpret_cast<const void*>(attn_f32_kernel), smem));
-  const long long items = static_cast<long long>(p.B) * p.H * p.S;
-  attn_f32_kernel<<<static_cast<unsigned int>((items + 3) / 4), 128, smem, st>>>(p);
-  CKL(h, "attn_f32_kernel");
-  return 0;
-}
-
-// Caption scoring's text rows (attention.cuh text_attn_wgmma_kernel): q / k / v [N * T, H * 64] back to back, image K / V
-// [B * M, H * 64]; out rows o_rs apart.
-static int launch_text_attention(gitb200_engine* h, const bf16* q, const bf16* k, const bf16* v, const bf16* img_k,
-                                 const bf16* img_v, int B, const TextAttnParams& ap, cudaStream_t st) {
-  TextAttnParams p = ap;
+// Text attention of caption scoring (attention.cuh): q / k / v [N * T, H * 64] (row n * T + t = position t of caption n)
+// back to back, image K / V [B * M, H * 64]; caption n attends to image image_index[n] (null: image n), img_lens (null, or
+// [B]) limits its keys.  bf16: text_attn_wgmma_kernel, out rows o_rs apart.  fp32 (parity mode): text_attn_f32_kernel, out
+// rows [hi | lo | hi] of 3 * H * 64 columns.
+struct TextAttn {
+  const void* q;
+  const void* k;
+  const void* v;
+  const void* img_k;
+  const void* img_v;
+  bf16* out;
+  int N, T, B, M, H;
+  long long o_rs;
+  const int* img_lens;
+  const int* image_index;
+};
+static int launch_text_attention(gitb200_engine* h, const TextAttn& a, bool fp32, cudaStream_t st) {
+  if (fp32) {
+    TextAttnF32Params p{};
+    p.q = static_cast<const float*>(a.q); p.k = static_cast<const float*>(a.k); p.v = static_cast<const float*>(a.v);
+    p.img_k = static_cast<const float*>(a.img_k); p.img_v = static_cast<const float*>(a.img_v); p.out = a.out;
+    p.N = a.N; p.T = a.T; p.H = a.H; p.d_model = a.H * 64; p.M = a.M; p.img_lens = a.img_lens; p.image_index = a.image_index;
+    const size_t smem = static_cast<size_t>(4) * (64 + p.M + p.T) * sizeof(float);
+    if (smem > 200 * 1024) return fail(h, "parity text attention: %d keys do not fit in shared memory", p.M + p.T);
+    TRY(set_dyn_smem(h, reinterpret_cast<const void*>(text_attn_f32_kernel), smem));
+    const long long items = static_cast<long long>(p.N) * p.H * p.T;
+    text_attn_f32_kernel<<<static_cast<unsigned int>((items + 3) / 4), 128, smem, st>>>(p);
+    CKL(h, "text_attn_f32_kernel");
+    return 0;
+  }
+  TextAttnParams p{};
+  p.out = a.out; p.N = a.N; p.T = a.T; p.H = a.H; p.M = a.M; p.img_lens = a.img_lens; p.image_index = a.image_index;
+  p.o_rs = a.o_rs;
   p.scale_log2 = 0.125f * 1.44269504088896340736f;
-  const long long rows = static_cast<long long>(ap.N) * ap.T, irows = static_cast<long long>(B) * ap.M, cols = ap.H * 64;
+  const long long rows = static_cast<long long>(a.N) * a.T, irows = static_cast<long long>(a.B) * a.M, cols = a.H * 64;
   CUtensorMap tq, tk, tv, tik, tiv;
-  TRY(get_tmap(h, q, rows, cols, cols, kAttnWgRows, &tq));
-  TRY(get_tmap(h, k, rows, cols, cols, kAttnWgRows, &tk));
-  TRY(get_tmap(h, v, rows, cols, cols, kAttnWgRows, &tv));
-  TRY(get_tmap(h, img_k, irows, cols, cols, kAttnWgRows, &tik));
-  TRY(get_tmap(h, img_v, irows, cols, cols, kAttnWgRows, &tiv));
-  const dim3 grid((ap.T + kAttnWgRows - 1) / kAttnWgRows, ap.H, ap.N);
+  TRY(get_tmap(h, a.q, rows, cols, cols, kAttnWgRows, &tq));
+  TRY(get_tmap(h, a.k, rows, cols, cols, kAttnWgRows, &tk));
+  TRY(get_tmap(h, a.v, rows, cols, cols, kAttnWgRows, &tv));
+  TRY(get_tmap(h, a.img_k, irows, cols, cols, kAttnWgRows, &tik));
+  TRY(get_tmap(h, a.img_v, irows, cols, cols, kAttnWgRows, &tiv));
+  const dim3 grid((a.T + kAttnWgRows - 1) / kAttnWgRows, a.H, a.N);
   text_attn_wgmma_kernel<<<grid, 128, kAttnWgSmem, st>>>(tq, tk, tv, tik, tiv, p);
   CKL(h, "text_attn_wgmma_kernel");
-  return 0;
-}
-
-static int launch_text_attention_f32(gitb200_engine* h, const TextAttnF32Params& p, cudaStream_t st) {
-  const size_t smem = static_cast<size_t>(4) * (64 + p.M + p.T) * sizeof(float);
-  if (smem > 200 * 1024) return fail(h, "parity text attention: %d keys do not fit in shared memory", p.M + p.T);
-  TRY(set_dyn_smem(h, reinterpret_cast<const void*>(text_attn_f32_kernel), smem));
-  const long long items = static_cast<long long>(p.N) * p.H * p.T;
-  text_attn_f32_kernel<<<static_cast<unsigned int>((items + 3) / 4), 128, smem, st>>>(p);
-  CKL(h, "text_attn_f32_kernel");
   return 0;
 }
 
@@ -550,11 +609,6 @@ static int launch_text_attention_f32(gitb200_engine* h, const TextAttnF32Params&
 // `items` (image, head) pairs.  The image K/V slice of one item is M rows of 128 B, staged in chunks of at most
 // kDecAttnChunk rows: two (K + V) staging buffers of one chunk per CTA, and at least two CTAs per SM (M = 257 in one piece
 // would be 131 KB per CTA = one 4-warp CTA per SM).  A uniform chunk is one TMA box.
-struct DecAttnGeom {
-  int chunk_rows, box_rows;   // DecAttnParams::chunk_rows / box_rows
-  size_t smem;                // dynamic shared memory per CTA
-  int grid;                   // CTAs the engine launches
-};
 static DecAttnGeom dec_attn_geometry(int M, const int* lens, int n, int num_sms, int items) {
   DecAttnGeom g;
   g.box_rows = g.chunk_rows = dec_attn_chunk_rows(M);
@@ -581,35 +635,78 @@ static int launch_decode_attn_inst(gitb200_engine* h, const DecAttnParams& ap, i
   CKL(h, "decode_attn_kernel");
   return 0;
 }
-// decode_attn_kernel<beam, ragged> on `grid` CTAs; ap.chunk_rows / box_rows and smem from dec_attn_geometry.
-static int launch_decode_attn(gitb200_engine* h, const DecAttnParams& ap, int beam, int grid, size_t smem, bool pdl,
-                              cudaStream_t st) {
-  CUtensorMap tk, tv;
-  TRY(get_tmap(h, ap.img_k, static_cast<long long>(ap.B) * ap.M, ap.D, ap.D, ap.box_rows, &tk, false));
-  TRY(get_tmap(h, ap.img_v, static_cast<long long>(ap.B) * ap.M, ap.D, ap.D, ap.box_rows, &tv, false));
-  const bool rg = ap.img_lens != nullptr;
-  switch (beam) {
-    case 1: return rg ? launch_decode_attn_inst<1, true>(h, ap, grid, smem, pdl, st, tk, tv)
-                      : launch_decode_attn_inst<1, false>(h, ap, grid, smem, pdl, st, tk, tv);
-    case 2: return rg ? launch_decode_attn_inst<2, true>(h, ap, grid, smem, pdl, st, tk, tv)
-                      : launch_decode_attn_inst<2, false>(h, ap, grid, smem, pdl, st, tk, tv);
-    case 3: return rg ? launch_decode_attn_inst<3, true>(h, ap, grid, smem, pdl, st, tk, tv)
-                      : launch_decode_attn_inst<3, false>(h, ap, grid, smem, pdl, st, tk, tv);
-    case 4: return rg ? launch_decode_attn_inst<4, true>(h, ap, grid, smem, pdl, st, tk, tv)
-                      : launch_decode_attn_inst<4, false>(h, ap, grid, smem, pdl, st, tk, tv);
-    default: return fail(h, "decode: beam size %d not supported (1 .. 4)", beam);
-  }
-}
 
-// decode_attn_f32_kernel (parity mode): one warp per (sequence, head); *ctas receives the grid.
-static int launch_decode_attn_f32(gitb200_engine* h, const DecAttnF32Params& ap, bool pdl, cudaStream_t st, unsigned int* ctas) {
-  const size_t smem = static_cast<size_t>(4) * dec_attn_f32_warp_floats(ap.M, ap.T_alloc) * sizeof(float);
-  if (smem > 200 * 1024) return fail(h, "parity decode attention: %d keys do not fit in shared memory", ap.M + ap.T_alloc);
-  TRY(set_dyn_smem(h, reinterpret_cast<const void*>(decode_attn_f32_kernel), smem));
-  *ctas = static_cast<unsigned int>((ap.R * (ap.D / 64) + 3) / 4);
-  CK(launch_k(pdl, decode_attn_f32_kernel, dim3(*ctas), dim3(128), smem, st, ap));
-  CKL(h, "decode_attn_f32_kernel");
-  return 0;
+// Decode-step attention (attention.cuh) of B images x beam rows at one text position (state->pos, or pos_fixed when state
+// is null): adds the QKV GEMM's n_partials split-K buffers and the bias, appends k / v to the text cache [R, T_alloc, D]
+// (rows through src_row when non-null) and attends to the image K/V [B, M, D] (img_lens: null, or [B] valid keys) and the
+// text keys so far.  bf16: decode_attn_kernel<beam, ragged> with geom from dec_attn_geometry.  fp32 (parity mode):
+// decode_attn_f32_kernel, one warp per (row, head), ctx rows [hi | lo | hi].  *ctas receives the grid.
+struct DecodeAttn {
+  const float* qkv;
+  int n_partials;
+  const float* bqkv;
+  const void* img_k;
+  const void* img_v;
+  void* txt_k;
+  void* txt_v;
+  const int* src_row;
+  bf16* ctx;
+  int B, beam, M, T_alloc, D;
+  const StepState* state;
+  int pos_fixed;
+  const int* img_lens;
+  DecAttnGeom geom;
+  ChainSync chain;
+  bool pdl;
+};
+static int launch_decode_attention(gitb200_engine* h, const DecodeAttn& a, bool fp32, cudaStream_t st, unsigned int* ctas) {
+  const int R = a.B * a.beam;
+  if (fp32) {
+    DecAttnF32Params p{};
+    p.qkv = a.qkv; p.n_partials = a.n_partials; p.partial_stride = static_cast<long long>(R) * 3 * a.D;
+    p.bqkv = a.bqkv;
+    p.img_k = static_cast<const float*>(a.img_k); p.img_v = static_cast<const float*>(a.img_v);
+    p.txt_k = static_cast<float*>(a.txt_k); p.txt_v = static_cast<float*>(a.txt_v);
+    p.src_row = a.src_row; p.ctx = a.ctx; p.R = R; p.beam = a.beam; p.M = a.M; p.T_alloc = a.T_alloc; p.D = a.D;
+    p.state = a.state; p.pos_fixed = a.pos_fixed;
+    p.chain = a.chain;
+    p.img_lens = a.img_lens;
+    const size_t smem = static_cast<size_t>(4) * dec_attn_f32_warp_floats(p.M, p.T_alloc) * sizeof(float);
+    if (smem > 200 * 1024) return fail(h, "parity decode attention: %d keys do not fit in shared memory", p.M + p.T_alloc);
+    TRY(set_dyn_smem(h, reinterpret_cast<const void*>(decode_attn_f32_kernel), smem));
+    *ctas = static_cast<unsigned int>((R * (p.D / 64) + 3) / 4);
+    CK(launch_k(a.pdl, decode_attn_f32_kernel, dim3(*ctas), dim3(128), smem, st, p));
+    CKL(h, "decode_attn_f32_kernel");
+    return 0;
+  }
+  DecAttnParams p{};
+  p.qkv = a.qkv; p.n_partials = a.n_partials; p.partial_stride = static_cast<long long>(R) * 3 * a.D;
+  p.bqkv = a.bqkv;
+  p.img_k = static_cast<const bf16*>(a.img_k); p.img_v = static_cast<const bf16*>(a.img_v);
+  p.txt_k = static_cast<bf16*>(a.txt_k); p.txt_v = static_cast<bf16*>(a.txt_v);
+  p.src_row = a.src_row; p.ctx = a.ctx; p.B = a.B; p.M = a.M; p.T_alloc = a.T_alloc; p.D = a.D;
+  p.state = a.state; p.pos_fixed = a.pos_fixed;
+  p.chunk_rows = a.geom.chunk_rows; p.box_rows = a.geom.box_rows;
+  p.chain = a.chain;
+  p.img_lens = a.img_lens;
+  CUtensorMap tk, tv;
+  TRY(get_tmap(h, a.img_k, static_cast<long long>(a.B) * a.M, a.D, a.D, a.geom.box_rows, &tk, false));
+  TRY(get_tmap(h, a.img_v, static_cast<long long>(a.B) * a.M, a.D, a.D, a.geom.box_rows, &tv, false));
+  const bool rg = a.img_lens != nullptr;
+  const int grid = a.geom.grid;
+  const size_t smem = a.geom.smem;
+  *ctas = static_cast<unsigned int>(grid);
+  switch (a.beam) {
+    case 1: return rg ? launch_decode_attn_inst<1, true>(h, p, grid, smem, a.pdl, st, tk, tv)
+                      : launch_decode_attn_inst<1, false>(h, p, grid, smem, a.pdl, st, tk, tv);
+    case 2: return rg ? launch_decode_attn_inst<2, true>(h, p, grid, smem, a.pdl, st, tk, tv)
+                      : launch_decode_attn_inst<2, false>(h, p, grid, smem, a.pdl, st, tk, tv);
+    case 3: return rg ? launch_decode_attn_inst<3, true>(h, p, grid, smem, a.pdl, st, tk, tv)
+                      : launch_decode_attn_inst<3, false>(h, p, grid, smem, a.pdl, st, tk, tv);
+    case 4: return rg ? launch_decode_attn_inst<4, true>(h, p, grid, smem, a.pdl, st, tk, tv)
+                      : launch_decode_attn_inst<4, false>(h, p, grid, smem, a.pdl, st, tk, tv);
+    default: return fail(h, "decode: beam size %d not supported (1 .. 4)", a.beam);
+  }
 }
 
 __global__ void cvt_rows_kernel(const float* __restrict__ src, long long src_ld, bf16* __restrict__ dst, long long dst_ld,
@@ -678,10 +775,8 @@ extern "C" int gitb200_set_option(gitb200_engine* h, const char* name, int64_t v
   drop_step_graphs(h);
   if (strcmp(name, "use_graph") == 0) { h->use_graph = value != 0; return 0; }
   if (strcmp(name, "use_pdl") == 0) { h->use_pdl = value != 0; return 0; }
-  if (strcmp(name, "use_chain") == 0) { h->use_chain = value != 0; return 0; }
   if (strcmp(name, "use_mega") == 0) { h->use_mega = value != 0; return 0; }
   if (strcmp(name, "debug_layers") == 0) { h->debug_layers = static_cast<int>(value); return 0; }
-  if (strcmp(name, "mega_coop") == 0) { h->mega_coop = value != 0; return 0; }
   if (strcmp(name, "parity") == 0) {
     if (h->weights_from != nullptr) return fail(h, "parity: this engine borrows its weights; switch the owning engine");
     if (h->parity != (value != 0)) { h->parity = value != 0; h->finalized = false; h->seen.clear(); h->tmaps.clear(); }
@@ -766,9 +861,8 @@ static void release_all(gitb200_engine* h) {
                     &h->pt, &h->pxd, &h->phd, &h->pq, &h->pctx, &h->pu, &h->img_kv, &h->txt_kv, &h->src_row[0],
                     &h->src_row[1], &h->xd_t, &h->hd_t, &h->qkv_t, &h->ctx_t, &h->t_t, &h->u_t, &h->logits, &h->state,
                     &h->next_token, &h->logprob_sum, &h->tokens_i64, &h->stage_img, &h->stage_tok, &h->stage_lp,
-                    &h->prefix_dev, &h->beam_ws, &h->sel_ws, &h->chain, &h->rg_tab, &h->rg_lens, &h->sc_t, &h->sc_x,
-                    &h->sc_h, &h->sc_q, &h->sc_kv, &h->sc_ctx, &h->sc_u, &h->sc_tgt, &h->sc_part, &h->sc_loss,
-                    &h->sc_valid, &h->sc_index};
+                    &h->prefix_dev, &h->beam_ws, &h->sel_ws, &h->chain, &h->rg_tab, &h->rg_lens, &h->sc_kv,
+                    &h->sc_tgt, &h->sc_part, &h->sc_loss, &h->sc_valid, &h->sc_index};
   for (DevBuf* b : bufs) b->release();
   for (auto& l : h->enc) {
     DevBuf* lb[] = {&l.wqkv, &l.bqkv, &l.wo, &l.bo, &l.ln1g, &l.ln1b, &l.ln2g, &l.ln2b, &l.w1, &l.b1, &l.w2, &l.b2};
@@ -1080,16 +1174,16 @@ static int encode_impl(gitb200_engine* h, const float* images, int B, int frames
   const long long Me = static_cast<long long>(NI) * L;
   const int ks = h->ks();                 // parity mode: GEMM operands are [hi | lo | hi] -> 3x the K extent
   const bool par = h->parity;
+  const size_t qkv_eb = h->kvb();         // q | k | v: bf16, fp32 in parity mode
   const int* seq_lens = rg ? h->rg_lens.as<int>() : nullptr;
   CK(h->x.ensure(Me * d * 4));
   CK(h->h.ensure(Me * d * 2 * ks));
-  CK(h->qkv.ensure(Me * 3 * d * (par ? 4 : 2)));         // parity: q | k | v stay fp32
+  CK(h->qkv.ensure(Me * 3 * d * qkv_eb));
   CK(h->ctx.ensure(Me * d * 2 * ks));
   CK(h->u.ensure(std::max<long long>(Me * 4 * d * 2, static_cast<long long>(NI) * (L - 1) * Kp * 2) * ks));
   CK(h->feats.ensure(Me * d * 2 * ks));
   float* x = h->x.as<float>();
   bf16* hb = h->h.as<bf16>();
-  bf16* qkv = h->qkv.as<bf16>();
   bf16* ctx = h->ctx.as<bf16>();
   bf16* u = h->u.as<bf16>();
 
@@ -1113,7 +1207,7 @@ static int encode_impl(gitb200_engine* h, const float* images, int B, int frames
     if (rg) im2col_patch_ragged_kernel<<<grid, 256, 0, st>>>(images, u, h->rg_tab.as<RaggedImg>(), NI, L - 1, h->cfg.patch, Kp, par ? 1 : 0);
     else im2col_patch_kernel<<<grid, 256, 0, st>>>(images, u, NI, h->in_h, h->in_w, h->cfg.patch, gh, gw, Kp, par ? 1 : 0);
     CKL(h, "im2col_patch_kernel");
-    GemmCall c = gemm_plain(u, Kp * ks, h->w_patch.as<bf16>(), Kp * ks, NI * (L - 1), d, Kp * ks, nullptr, ACT_NONE, nullptr, x, false);
+    GemmCall c = gemm_rows(h, RowOut::F32, u, h->w_patch.as<bf16>(), NI * (L - 1), d, Kp, nullptr, ACT_NONE, nullptr, x);
     c.p.rows_per_batch = L - 1;
     c.p.batch_stride = L;
     c.p.row_offset = 1;
@@ -1130,50 +1224,30 @@ static int encode_impl(gitb200_engine* h, const float* images, int B, int frames
       cls_pos_lnpre_kernel<1024><<<gridr, 256, 0, st>>>(x, h->cls.as<float>(), pos, h->lnpre_g.as<float>(), h->lnpre_b.as<float>(), static_cast<int>(Me), L);
     CKL(h, "cls_pos_lnpre_kernel");
   }
-  auto ln_enc = [&](const float* g, const float* b) {
-    LnParams p = ln_params(x, nullptr, nullptr, g, b, 1e-5f, nullptr, hb, static_cast<int>(Me));
-    p.split3 = par ? 1 : 0;
-    return p;
-  };
+  const int rows = static_cast<int>(Me);
+  const char* qkv = h->qkv.as<char>();
+  SelfAttn attn{};
+  attn.q = qkv; attn.k = qkv + d * qkv_eb; attn.v = qkv + 2 * d * qkv_eb; attn.out = ctx;
+  attn.B = NI; attn.S = L; attn.H = H;
+  attn.q_rs = attn.kv_rs = 3 * d; attn.q_bs = attn.kv_bs = static_cast<long long>(L) * 3 * d;
+  attn.o_rs = d * ks; attn.o_bs = static_cast<long long>(L) * attn.o_rs;
+  attn.seq_lens = seq_lens;
   for (int i = 0; i < h->cfg.enc_layers; ++i) {
     EncLayer& l = h->enc[i];
-    TRY(launch_ln(h, ln_enc(l.ln1g.as<float>(), l.ln1b.as<float>()), d, st));
-    TRY(launch_gemm(h, gemm_plain(hb, d * ks, l.wqkv.as<bf16>(), d * ks, static_cast<int>(Me), 3 * d, d * ks, l.bqkv.as<float>(), ACT_NONE, nullptr, qkv, !par), st));
-    if (par) {
-      AttnF32Params ap{};
-      const float* qf = h->qkv.as<float>();
-      ap.q = qf; ap.k = qf + d; ap.v = qf + 2 * d; ap.out = ctx;
-      ap.B = NI; ap.S = L; ap.H = H; ap.d_model = d;
-      ap.q_rs = 3 * d; ap.kv_rs = 3 * d; ap.q_bs = static_cast<long long>(L) * 3 * d; ap.kv_bs = ap.q_bs;
-      ap.o_bs = static_cast<long long>(L) * 3 * d;
-      ap.seq_lens = seq_lens;
-      TRY(launch_attention_f32(h, ap, st));
-    } else {
-      AttnParams ap{};
-      ap.q = qkv; ap.k = qkv + d; ap.v = qkv + 2 * d; ap.out = ctx;
-      ap.B = NI; ap.S = L; ap.H = H;
-      ap.q_rs = 3 * d; ap.kv_rs = 3 * d; ap.q_bs = static_cast<long long>(L) * 3 * d; ap.kv_bs = ap.q_bs;
-      ap.o_rs = d; ap.o_bs = static_cast<long long>(L) * d;
-      ap.seq_lens = seq_lens;
-      TRY(launch_attention(h, ap, st));
-    }
-    TRY(launch_gemm(h, gemm_plain(ctx, d * ks, l.wo.as<bf16>(), d * ks, static_cast<int>(Me), d, d * ks, l.bo.as<float>(), ACT_NONE, x, x, false), st));
-    TRY(launch_ln(h, ln_enc(l.ln2g.as<float>(), l.ln2b.as<float>()), d, st));
-    {
-      GemmCall c = gemm_plain(hb, d * ks, l.w1.as<bf16>(), d * ks, static_cast<int>(Me), 4 * d, d * ks, l.b1.as<float>(),
-                              par ? ACT_QUICKGELU_EXACT : ACT_QUICKGELU, nullptr, u, true);
-      if (par) { c.p.split3 = 1; c.p.ldo = 3LL * 4 * d; }
-      TRY(launch_gemm(h, c, st));
-    }
-    TRY(launch_gemm(h, gemm_plain(u, 4 * d * ks, l.w2.as<bf16>(), 4 * d * ks, static_cast<int>(Me), d, 4 * d * ks, l.b2.as<float>(), ACT_NONE, x, x, false), st));
+    TRY(launch_ln(h, ln_operand(h, x, l.ln1g.as<float>(), l.ln1b.as<float>(), 1e-5f, nullptr, hb, rows), d, st));
+    TRY(launch_gemm(h, gemm_rows(h, RowOut::QKV, hb, l.wqkv.as<bf16>(), rows, 3 * d, d, l.bqkv.as<float>(), ACT_NONE, nullptr, h->qkv.p), st));
+    TRY(launch_self_attention(h, attn, par, st));
+    TRY(launch_gemm(h, gemm_rows(h, RowOut::F32, ctx, l.wo.as<bf16>(), rows, d, d, l.bo.as<float>(), ACT_NONE, x, x), st));
+    TRY(launch_ln(h, ln_operand(h, x, l.ln2g.as<float>(), l.ln2b.as<float>(), 1e-5f, nullptr, hb, rows), d, st));
+    TRY(launch_gemm(h, gemm_rows(h, RowOut::OPERAND, hb, l.w1.as<bf16>(), rows, 4 * d, d, l.b1.as<float>(), ACT_QUICKGELU, nullptr, u), st));
+    TRY(launch_gemm(h, gemm_rows(h, RowOut::F32, u, l.w2.as<bf16>(), rows, d, 4 * d, l.b2.as<float>(), ACT_NONE, x, x), st));
   }
   // ln_post on all tokens (+ temporal embedding), re-ordered to [B, frames*L, d]
   {
-    LnParams p = ln_params(x, nullptr, nullptr, h->lnpost_g.as<float>(), h->lnpost_b.as<float>(), 1e-5f, feats_out, h->feats.as<bf16>(), static_cast<int>(Me));
+    LnParams p = ln_operand(h, x, h->lnpost_g.as<float>(), h->lnpost_b.as<float>(), 1e-5f, feats_out, h->feats.as<bf16>(), rows);
     p.remap_B = B; p.remap_F = frames; p.remap_L = L;
     // temporal embeddings only for list inputs (reference layers/decoder.py:846-849; a bare tensor skips them)
     p.temb = (list_input && h->cfg.num_frames_emb > 0) ? h->temb.as<float>() : nullptr;
-    p.split3 = par ? 1 : 0;
     TRY(launch_ln(h, p, d, st));
   }
   h->cur_B = B;
@@ -1201,10 +1275,12 @@ static char* txt_kv_ptr(gitb200_engine* h, int layer, int kv, long long elem_off
   return h->txt_kv.as<char>() + ((static_cast<long long>(layer) * 2 + kv) * per + elem_off) * h->kvb();
 }
 
-// Workspaces of the image rows of the decoder (visual projection + layers) and the image K/V cache of the last encode.
-static int image_rows_buffers(gitb200_engine* h) {
+// Workspaces of the decoder-layer pass for the image rows of the last encode and `text_rows` further rows (the larger of
+// the two), and the image K/V cache.  Sized before a call's first launch: DevBuf::ensure frees the buffer it replaces.
+static int decoder_buffers(gitb200_engine* h, long long text_rows) {
   const int D = h->D, F = h->F, nl = h->cfg.dec_layers;
-  const long long rows = static_cast<long long>(h->cur_B) * h->cur_M;
+  const long long img_rows = static_cast<long long>(h->cur_B) * h->cur_M;
+  const long long rows = std::max(img_rows, text_rows);
   const int ks = h->ks();
   const long long kvb = static_cast<long long>(h->kvb());
   CK(h->pt.ensure(rows * D * 4));
@@ -1213,10 +1289,70 @@ static int image_rows_buffers(gitb200_engine* h) {
   CK(h->pq.ensure(rows * D * kvb));
   CK(h->pctx.ensure(rows * D * 2 * ks));
   CK(h->pu.ensure(rows * F * 2 * ks));
-  CK(h->img_kv.ensure(static_cast<long long>(nl) * 2 * rows * D * kvb));
+  CK(h->img_kv.ensure(static_cast<long long>(nl) * 2 * img_rows * D * kvb));
   return 0;
 }
-static int image_rows(gitb200_engine* h, float* vproj_out, cudaStream_t st);
+
+// The decoder layers (post-LN, erf-GELU) over `rows` rows whose input is in pxd (fp32) and phd (GEMM operand).  Layer j's
+// k / v rows go to kv: [layer][k|v][rows][D] when kv_per_layer (the image K/V cache), else every layer overwrites the one
+// [k|v][rows][D] pair there.  attend(j, q, k, v, ctx) launches layer j's attention.  last_qkv_only: the last layer stops
+// after its QKV GEMM (only its k / v are read).  Buffers from decoder_buffers.
+template <typename Attend>
+static int decoder_layers(gitb200_engine* h, int rows, char* kv, bool kv_per_layer, bool last_qkv_only, Attend&& attend,
+                          cudaStream_t st) {
+  const int D = h->D, F = h->F, nl = h->cfg.dec_layers;
+  const long long kv_bytes = static_cast<long long>(rows) * D * h->kvb();   // one k or v block
+  float* t = h->pt.as<float>();
+  float* xd = h->pxd.as<float>();
+  bf16* hd = h->phd.as<bf16>();
+  bf16* ctx = h->pctx.as<bf16>();
+  bf16* u = h->pu.as<bf16>();
+  auto ln = [&](const DevBuf& g, const DevBuf& b) {
+    return launch_ln(h, ln_operand(h, t, g.as<float>(), b.as<float>(), 1e-12f, xd, hd, rows), D, st);
+  };
+  for (int j = 0; j < nl; ++j) {
+    DecLayer& l = h->dec[j];
+    char* k = kv + (kv_per_layer ? 2 * j * kv_bytes : 0);
+    char* v = k + kv_bytes;
+    GemmCall c = gemm_rows(h, RowOut::QKV, hd, l.wqkv.as<bf16>(), rows, 3 * D, D, l.bqkv.as<float>(), ACT_NONE, nullptr, h->pq.p);
+    c.p.seg_n = D;
+    c.p.out[1] = k; c.p.out[2] = v;
+    c.p.ldo = D;
+    TRY(launch_gemm(h, c, st));
+    if (last_qkv_only && j + 1 == nl) break;
+    TRY(attend(j, h->pq.p, k, v, ctx));
+    TRY(launch_gemm(h, gemm_rows(h, RowOut::F32, ctx, l.wo.as<bf16>(), rows, D, D, l.bo.as<float>(), ACT_NONE, xd, t), st));
+    TRY(ln(l.lnag, l.lnab));
+    TRY(launch_gemm(h, gemm_rows(h, RowOut::OPERAND, hd, l.w1.as<bf16>(), rows, F, D, l.b1.as<float>(), ACT_GELU_ERF, nullptr, u), st));
+    TRY(launch_gemm(h, gemm_rows(h, RowOut::F32, u, l.w2.as<bf16>(), rows, D, F, l.b2.as<float>(), ACT_NONE, xd, t), st));
+    TRY(ln(l.lnog, l.lnob));
+  }
+  return 0;
+}
+
+// The image rows of the decoder, computed once per encode: visual projection, then the layers over the image rows only
+// (they never attend to text, reference layers/decoder.py:119-120), whose k / v rows fill the image K/V cache.  Buffers
+// from decoder_buffers.
+static int image_rows(gitb200_engine* h, float* vproj_out, cudaStream_t st) {
+  const int D = h->D, d = h->d, M = h->cur_M, B = h->cur_B;
+  const int rows = B * M;
+  float* t = h->pt.as<float>();
+  float* xd = h->pxd.as<float>();
+  // visual projection: Linear(dv -> 768) + LayerNorm(1e-5)
+  TRY(launch_gemm(h, gemm_rows(h, RowOut::F32, h->feats.as<bf16>(), h->w_vp.as<bf16>(), rows, D, d, h->b_vp.as<float>(), ACT_NONE, nullptr, t), st));
+  TRY(launch_ln(h, ln_operand(h, t, h->lnvp_g.as<float>(), h->lnvp_b.as<float>(), 1e-5f, xd, h->phd.as<bf16>(), rows), D, st));
+  if (vproj_out) CK(cudaMemcpyAsync(vproj_out, xd, static_cast<size_t>(rows) * D * 4, cudaMemcpyDeviceToDevice, st));
+  SelfAttn a{};
+  a.B = B; a.S = M; a.H = h->cfg.dec_heads;
+  a.q_rs = a.kv_rs = D; a.q_bs = a.kv_bs = static_cast<long long>(M) * D;
+  a.o_rs = D * h->ks(); a.o_bs = static_cast<long long>(M) * a.o_rs;
+  a.seq_lens = h->cur_ragged ? h->rg_lens.as<int>() : nullptr;
+  auto self_attention = [&](int, const void* q, const void* k, const void* v, bf16* ctx) {
+    a.q = q; a.k = k; a.v = v; a.out = ctx;
+    return launch_self_attention(h, a, h->parity, st);
+  };
+  return decoder_layers(h, rows, h->img_kv.as<char>(), true, true, self_attention, st);
+}
 
 static int prefill_impl(gitb200_engine* h, int B, int beam, int T_alloc, float* vproj_out, cudaStream_t st) {
   if (B != h->cur_B || h->cur_M <= 0) return fail(h, "prefill: call encode with the same batch first");
@@ -1224,7 +1360,7 @@ static int prefill_impl(gitb200_engine* h, int B, int beam, int T_alloc, float* 
   const int R = B * beam;
   const int ks = h->ks();
   const long long kvb = static_cast<long long>(h->kvb());
-  TRY(image_rows_buffers(h));
+  TRY(decoder_buffers(h, 0));
   {
     // decode_mega_kernel fetches the text cache in 16-position steps up to the caption's end and masks the positions past
     // it in the last step by giving them probability 0 -- which only works if what lies there is finite: a fresh allocation is zeroed once
@@ -1256,75 +1392,14 @@ static int prefill_impl(gitb200_engine* h, int B, int beam, int T_alloc, float* 
   return image_rows(h, vproj_out, st);
 }
 
-// The image rows of the decoder, computed once per encode: visual projection, then the layers over the image rows only
-// (they never attend to text, reference layers/decoder.py:119-120), whose k / v rows fill the image K/V cache.  Buffers
-// from image_rows_buffers.
-static int image_rows(gitb200_engine* h, float* vproj_out, cudaStream_t st) {
-  const int D = h->D, F = h->F, d = h->d, M = h->cur_M, B = h->cur_B, nl = h->cfg.dec_layers, H = h->cfg.dec_heads;
-  const long long rows = static_cast<long long>(B) * M;
-  const int ks = h->ks();
-  const bool par = h->parity;
-  float* t = h->pt.as<float>();
-  float* xd = h->pxd.as<float>();
-  bf16* hd = h->phd.as<bf16>();
-  bf16* q = h->pq.as<bf16>();
-  bf16* ctx = h->pctx.as<bf16>();
-  bf16* u = h->pu.as<bf16>();
-
-  auto ln_pre = [&](const float* g, const float* b, float eps) {
-    LnParams p = ln_params(t, nullptr, nullptr, g, b, eps, xd, hd, static_cast<int>(rows));
-    p.split3 = par ? 1 : 0;
-    return p;
-  };
-  // visual projection: Linear(dv -> 768) + LayerNorm(1e-5)
-  TRY(launch_gemm(h, gemm_plain(h->feats.as<bf16>(), d * ks, h->w_vp.as<bf16>(), d * ks, static_cast<int>(rows), D, d * ks, h->b_vp.as<float>(), ACT_NONE, nullptr, t, false), st));
-  TRY(launch_ln(h, ln_pre(h->lnvp_g.as<float>(), h->lnvp_b.as<float>(), 1e-5f), D, st));
-  if (vproj_out) CK(cudaMemcpyAsync(vproj_out, xd, rows * D * 4, cudaMemcpyDeviceToDevice, st));
-  for (int j = 0; j < nl; ++j) {
-    DecLayer& l = h->dec[j];
-    // fused q|k|v projection; k and v rows go straight into the image K/V cache (bf16; fp32 in parity mode)
-    GemmCall c = gemm_plain(hd, D * ks, l.wqkv.as<bf16>(), D * ks, static_cast<int>(rows), 3 * D, D * ks, l.bqkv.as<float>(), ACT_NONE, nullptr, q, !par);
-    c.p.seg_n = D;
-    c.p.out[0] = q; c.p.out[1] = img_kv_ptr(h, j, 0); c.p.out[2] = img_kv_ptr(h, j, 1);
-    c.p.ldo = D;
-    TRY(launch_gemm(h, c, st));
-    if (j + 1 == nl) break;  // image rows of the last layer are never read (text rows only need their K/V)
-    if (par) {
-      AttnF32Params ap{};
-      ap.q = h->pq.as<float>(); ap.k = reinterpret_cast<const float*>(img_kv_ptr(h, j, 0));
-      ap.v = reinterpret_cast<const float*>(img_kv_ptr(h, j, 1)); ap.out = ctx;
-      ap.B = B; ap.S = M; ap.H = H; ap.d_model = D;
-      ap.q_rs = D; ap.kv_rs = D; ap.q_bs = static_cast<long long>(M) * D; ap.kv_bs = ap.q_bs; ap.o_bs = 3 * ap.q_bs;
-      ap.seq_lens = h->cur_ragged ? h->rg_lens.as<int>() : nullptr;
-      TRY(launch_attention_f32(h, ap, st));
-    } else {
-      AttnParams ap{};
-      ap.q = q; ap.k = reinterpret_cast<const bf16*>(img_kv_ptr(h, j, 0)); ap.v = reinterpret_cast<const bf16*>(img_kv_ptr(h, j, 1)); ap.out = ctx;
-      ap.B = B; ap.S = M; ap.H = H;
-      ap.q_rs = D; ap.kv_rs = D; ap.q_bs = static_cast<long long>(M) * D; ap.kv_bs = ap.q_bs; ap.o_rs = D; ap.o_bs = ap.q_bs;
-      ap.seq_lens = h->cur_ragged ? h->rg_lens.as<int>() : nullptr;
-      TRY(launch_attention(h, ap, st));
-    }
-    TRY(launch_gemm(h, gemm_plain(ctx, D * ks, l.wo.as<bf16>(), D * ks, static_cast<int>(rows), D, D * ks, l.bo.as<float>(), ACT_NONE, xd, t, false), st));
-    TRY(launch_ln(h, ln_pre(l.lnag.as<float>(), l.lnab.as<float>(), 1e-12f), D, st));
-    {
-      GemmCall c1 = gemm_plain(hd, D * ks, l.w1.as<bf16>(), D * ks, static_cast<int>(rows), F, D * ks, l.b1.as<float>(), ACT_GELU_ERF, nullptr, u, true);
-      if (par) { c1.p.split3 = 1; c1.p.ldo = 3LL * F; }
-      TRY(launch_gemm(h, c1, st));
-    }
-    TRY(launch_gemm(h, gemm_plain(u, F * ks, l.w2.as<bf16>(), F * ks, static_cast<int>(rows), D, F * ks, l.b2.as<float>(), ACT_NONE, xd, t, false), st));
-    TRY(launch_ln(h, ln_pre(l.lnog.as<float>(), l.lnob.as<float>(), 1e-12f), D, st));
-  }
-  return 0;
-}
-
-// One decode step for the `rows` sequences: embed next_token at state->pos, 6 layers against the KV caches,
+// One decode step for the cur_rows sequences: embed next_token at state->pos, 6 layers against the KV caches,
 // optional LM head -> h->logits.  Every kernel reads the position / finished flag from device state so the
-// same launch sequence (and CUDA graph) serves every step.
-static int step_layers(gitb200_engine* h, Lane& ln_, const long long* tokens, const int* src_row, bool lm_head) {
-  const int D = h->D, F = h->F, R = ln_.rows, beam = h->cur_beam;
+// same launch sequence (and CUDA graph) serves every step.  *tail (optional) receives the chain position of the last
+// kernel launched, for the selection kernel that follows.
+static int step_layers(gitb200_engine* h, cudaStream_t st, const long long* tokens, const int* src_row, bool lm_head,
+                       ChainSync* tail = nullptr) {
+  const int D = h->D, F = h->F, R = h->cur_rows, beam = h->cur_beam;
   const int nl = (h->debug_layers >= 0) ? std::min(h->debug_layers, h->cfg.dec_layers) : h->cfg.dec_layers;
-  cudaStream_t st = ln_.st;
   StepState* state = h->state.as<StepState>();
   const int* skip = &state->finished;
   const int ks = h->ks();
@@ -1338,7 +1413,7 @@ static int step_layers(gitb200_engine* h, Lane& ln_, const long long* tokens, co
   float* logits = h->logits.as<float>();
   const bool pdl = h->use_pdl;
   // Ordering inside the step: flag chain (greedy; the beam bookkeeping kernels still use grid dependencies).
-  const bool chain_on = pdl && h->use_chain && beam == 1;
+  const bool chain_on = pdl && beam == 1;
   ChainSync cs{};
   cs.counters = chain_on ? h->chain.as<unsigned int>() : nullptr;
   cs.idx = 0;
@@ -1368,6 +1443,14 @@ static int step_layers(gitb200_engine* h, Lane& ln_, const long long* tokens, co
     p.split3 = par ? 1 : 0;
     return p;
   };
+  DecodeAttn da{};
+  da.n_partials = kQkvSplits;
+  da.src_row = src_row; da.ctx = ctx;
+  da.B = h->cur_B; da.beam = beam; da.M = h->cur_M; da.T_alloc = h->T_alloc; da.D = D;
+  da.state = state;
+  da.img_lens = h->cur_ragged ? h->rg_lens.as<int>() : nullptr;
+  da.geom = h->attn_geom;
+  da.pdl = pdl;
   auto ln = [&](LnParams p) -> int {
     p.skip_flag = skip; p.chain = cs;
     TRY(launch_ln(h, p, D, st, pdl));
@@ -1377,34 +1460,13 @@ static int step_layers(gitb200_engine* h, Lane& ln_, const long long* tokens, co
   for (int j = 0; j < nl; ++j) {
     DecLayer& l = h->dec[j];
     TRY(skinny(gemm_skinny(hd, D * ks, l.wqkv.as<bf16>(), D * ks, R, 3 * D, D * ks, nullptr, ACT_NONE, qkv, 3 * D, false, kQkvSplits, skip, pdl)));
-    if (par) {
-      DecAttnF32Params ap{};
-      ap.qkv = qkv; ap.n_partials = kQkvSplits; ap.partial_stride = static_cast<long long>(R) * 3 * D;
-      ap.bqkv = l.bqkv.as<float>();
-      ap.img_k = reinterpret_cast<const float*>(img_kv_ptr(h, j, 0)); ap.img_v = reinterpret_cast<const float*>(img_kv_ptr(h, j, 1));
-      ap.txt_k = reinterpret_cast<float*>(txt_kv_ptr(h, j, 0)); ap.txt_v = reinterpret_cast<float*>(txt_kv_ptr(h, j, 1));
-      ap.src_row = src_row; ap.ctx = ctx; ap.R = R; ap.beam = beam; ap.M = h->cur_M; ap.T_alloc = h->T_alloc; ap.D = D;
-      ap.state = state;
-      ap.chain = cs;
-      ap.img_lens = h->cur_ragged ? h->rg_lens.as<int>() : nullptr;
-      unsigned int grid = 0;
-      TRY(launch_decode_attn_f32(h, ap, pdl, st, &grid));
-      next_link(grid);
-    } else {
-      DecAttnParams ap{};
-      ap.qkv = qkv; ap.n_partials = kQkvSplits; ap.partial_stride = static_cast<long long>(R) * 3 * D;
-      ap.bqkv = l.bqkv.as<float>();
-      ap.img_k = reinterpret_cast<const bf16*>(img_kv_ptr(h, j, 0)); ap.img_v = reinterpret_cast<const bf16*>(img_kv_ptr(h, j, 1));
-      ap.txt_k = reinterpret_cast<bf16*>(txt_kv_ptr(h, j, 0)); ap.txt_v = reinterpret_cast<bf16*>(txt_kv_ptr(h, j, 1));
-      ap.src_row = src_row; ap.ctx = ctx; ap.B = ln_.nb; ap.M = h->cur_M; ap.T_alloc = h->T_alloc; ap.D = D;
-      ap.state = state;
-      ap.chunk_rows = h->attn_chunk_rows; ap.box_rows = h->attn_box_rows;
-      ap.chain = cs;
-      ap.img_lens = h->cur_ragged ? h->rg_lens.as<int>() : nullptr;
-      const int grid = std::min(h->attn_grid, ln_.nb * h->cfg.dec_heads);
-      TRY(launch_decode_attn(h, ap, beam, grid, h->attn_smem, pdl, st));
-      next_link(static_cast<unsigned int>(grid));
-    }
+    da.qkv = qkv; da.bqkv = l.bqkv.as<float>();
+    da.img_k = img_kv_ptr(h, j, 0); da.img_v = img_kv_ptr(h, j, 1);
+    da.txt_k = txt_kv_ptr(h, j, 0); da.txt_v = txt_kv_ptr(h, j, 1);
+    da.chain = cs;
+    unsigned int ctas = 0;
+    TRY(launch_decode_attention(h, da, par, st, &ctas));
+    next_link(ctas);
     TRY(skinny(gemm_skinny(ctx, D * ks, l.wo.as<bf16>(), D * ks, R, D, D * ks, nullptr, ACT_NONE, t, D, false, kOutProjSplits, skip, pdl)));
     TRY(ln(ln_partials(t, kOutProjSplits, R, l.bo.as<float>(), xd, l.lnag.as<float>(), l.lnab.as<float>(), xd, hd)));
     {
@@ -1417,19 +1479,14 @@ static int step_layers(gitb200_engine* h, Lane& ln_, const long long* tokens, co
   }
   if (lm_head)
     TRY(skinny(gemm_skinny(hd, D * ks, h->words_bf16.as<bf16>(), D * ks, R, h->V, D * ks, h->out_bias.as<float>(), ACT_NONE, logits, h->V, false, 1, skip, pdl)));
-  ln_.chain_idx = cs.idx;
-  ln_.chain_ctas = cs.pred_ctas;
+  if (tail) *tail = cs;
   return 0;
 }
 
 // Decode-attention geometry of the last prefill (dec_attn_geometry) and the step chain's counters.
 static int set_decode_geometry(gitb200_engine* h) {
-  const DecAttnGeom g = dec_attn_geometry(h->cur_M, h->cur_ragged ? h->cur_lens.data() : nullptr, h->cur_B, h->num_sms,
-                                          h->cur_B * h->cfg.dec_heads);
-  h->attn_chunk_rows = g.chunk_rows;
-  h->attn_box_rows = g.box_rows;
-  h->attn_smem = g.smem;
-  h->attn_grid = g.grid;
+  h->attn_geom = dec_attn_geometry(h->cur_M, h->cur_ragged ? h->cur_lens.data() : nullptr, h->cur_B, h->num_sms,
+                                   h->cur_B * h->cfg.dec_heads);
   CK(h->chain.ensure(256));
   CK(cudaMemset(h->chain.p, 0, 256));
   return 0;

@@ -41,6 +41,47 @@ struct LnParams {
   ChainSync chain;       // decode-step flag ordering (counters == null: plain / PDL ordering)
 };
 
+// The LayerNorm row routine of every LN kernel below: one warp holds a row of D floats as NV = D / 128 float4 per lane.
+// Two-pass statistics: the mean, then rsqrtf(biased variance + eps).
+template <int D>
+__device__ __forceinline__ void ln_row_stats(const float4 (&v)[D / 128], float eps, float& mean, float& rstd) {
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < D / 128; ++i) s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
+  mean = warp_sum(s) * (1.0f / D);
+  float ss = 0.f;
+#pragma unroll
+  for (int i = 0; i < D / 128; ++i) {
+    const float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
+    ss += (a * a + b * b) + (c * c + d * d);
+  }
+  rstd = rsqrtf(warp_sum(ss) * (1.0f / D) + eps);
+}
+// One float4 of the normalised row.
+__device__ __forceinline__ float4 ln_norm(const float4 v, float mean, float rstd, const float4 g, const float4 b) {
+  return make_float4((v.x - mean) * rstd * g.x + b.x, (v.y - mean) * rstd * g.y + b.y, (v.z - mean) * rstd * g.z + b.z,
+                     (v.w - mean) * rstd * g.w + b.w);
+}
+// Stores float4 k (= i * 32 + lane) of output row `row`: fp32 to out_f32, and bf16 to out_bf16, or [hi | lo | hi] rows of
+// 3 D there when split3 (parity mode's GEMM operand format, see split_bf16 in ptx.cuh).  A null output is skipped.
+template <int D>
+__device__ __forceinline__ void ln_store(float* out_f32, __nv_bfloat16* out_bf16, int split3, long long row, int k,
+                                         const float4 o) {
+  if (out_f32 != nullptr) reinterpret_cast<float4*>(out_f32 + row * D)[k] = o;
+  if (out_bf16 != nullptr && split3) {
+    uint2 hi, lo;
+    pack_split2(o.x, o.y, hi.x, lo.x);
+    pack_split2(o.z, o.w, hi.y, lo.y);
+    uint2* dst = reinterpret_cast<uint2*>(out_bf16 + row * 3 * D) + k;
+    dst[0] = hi; dst[D / 4] = lo; dst[D / 2] = hi;
+  } else if (out_bf16 != nullptr) {
+    uint2 pk;
+    pk.x = pack_bf16(o.x, o.y);
+    pk.y = pack_bf16(o.z, o.w);
+    reinterpret_cast<uint2*>(out_bf16 + row * D)[k] = pk;
+  }
+}
+
 // PRE: fetch gamma / beta / bias before the dependency wait (decode chain: hides one L2 round trip; costs registers,
 // so the big encoder LayerNorms use PRE = false).
 template <int D, bool PRE>
@@ -113,17 +154,8 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const LnParams p) {
       v[i].x += b.x; v[i].y += b.y; v[i].z += b.z; v[i].w += b.w;
     }
   }
-  float s = 0.f;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
-  const float mean = warp_sum(s) * (1.0f / D);
-  float ss = 0.f;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
-    ss += (a * a + b * b) + (c * c + d * d);
-  }
-  const float rstd = rsqrtf(warp_sum(ss) * (1.0f / D) + p.eps);
+  float mean, rstd;
+  ln_row_stats<D>(v, p.eps, mean, rstd);
 
   long long orow = row;
   int frame = 0;
@@ -138,28 +170,12 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const LnParams p) {
   for (int i = 0; i < NV; ++i) {
     const float4 g = PRE ? gam[i] : __ldg(reinterpret_cast<const float4*>(p.gamma) + i * 32 + lane);
     const float4 b = PRE ? bet[i] : __ldg(reinterpret_cast<const float4*>(p.beta) + i * 32 + lane);
-    float4 o;
-    o.x = (v[i].x - mean) * rstd * g.x + b.x;
-    o.y = (v[i].y - mean) * rstd * g.y + b.y;
-    o.z = (v[i].z - mean) * rstd * g.z + b.z;
-    o.w = (v[i].w - mean) * rstd * g.w + b.w;
+    float4 o = ln_norm(v[i], mean, rstd, g, b);
     if (p.temb != nullptr) {
       const float4 t = __ldg(reinterpret_cast<const float4*>(p.temb + static_cast<long long>(frame) * D) + i * 32 + lane);
       o.x += t.x; o.y += t.y; o.z += t.z; o.w += t.w;
     }
-    if (p.out_f32 != nullptr) reinterpret_cast<float4*>(p.out_f32 + orow * D)[i * 32 + lane] = o;
-    if (p.out_bf16 != nullptr && p.split3) {
-      uint2 hi, lo;
-      pack_split2(o.x, o.y, hi.x, lo.x);
-      pack_split2(o.z, o.w, hi.y, lo.y);
-      uint2* dst = reinterpret_cast<uint2*>(p.out_bf16 + orow * 3 * D) + i * 32 + lane;
-      dst[0] = hi; dst[D / 4] = lo; dst[D / 2] = hi;
-    } else if (p.out_bf16 != nullptr) {
-      uint2 pk;
-      pk.x = pack_bf16(o.x, o.y);
-      pk.y = pack_bf16(o.z, o.w);
-      reinterpret_cast<uint2*>(p.out_bf16 + orow * D)[i * 32 + lane] = pk;
-    }
+    ln_store<D>(p.out_f32, p.out_bf16, p.split3, orow, i * 32 + lane, o);
   }
   tl_mark(200002);
   chain_signal(p.chain);
@@ -352,29 +368,20 @@ cls_pos_lnpre_kernel(float* __restrict__ x, const float* __restrict__ cls, const
   const float4* src = (l == 0) ? reinterpret_cast<const float4*>(cls)
                                : reinterpret_cast<const float4*>(x + static_cast<long long>(row) * D);
   const float4* pp = reinterpret_cast<const float4*>(pos + static_cast<long long>(l) * D);
-  float s = 0.f;
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const float4 a = src[i * 32 + lane];
     const float4 b = __ldg(pp + i * 32 + lane);
     v[i] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
-    s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
   }
-  const float mean = warp_sum(s) * (1.0f / D);
-  float ss = 0.f;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
-    ss += (a * a + b * b) + (c * c + d * d);
-  }
-  const float rstd = rsqrtf(warp_sum(ss) * (1.0f / D) + 1e-5f);
+  float mean, rstd;
+  ln_row_stats<D>(v, 1e-5f, mean, rstd);
   float4* op = reinterpret_cast<float4*>(x + static_cast<long long>(row) * D);
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const float4 g = __ldg(reinterpret_cast<const float4*>(gamma) + i * 32 + lane);
     const float4 b = __ldg(reinterpret_cast<const float4*>(beta) + i * 32 + lane);
-    op[i * 32 + lane] = make_float4((v[i].x - mean) * rstd * g.x + b.x, (v[i].y - mean) * rstd * g.y + b.y,
-                                    (v[i].z - mean) * rstd * g.z + b.z, (v[i].w - mean) * rstd * g.w + b.w);
+    op[i * 32 + lane] = ln_norm(v[i], mean, rstd, g, b);
   }
 }
 
@@ -403,41 +410,20 @@ embed_ln_kernel(const long long* __restrict__ tokens, long long tok_stride, cons
   const float4* wp = reinterpret_cast<const float4*>(words + tok * D);
   const float4* pp = reinterpret_cast<const float4*>(positions + static_cast<long long>(pos) * D);
   float4 v[NV];
-  float s = 0.f;
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const float4 a = __ldg(wp + i * 32 + lane);
     const float4 b = __ldg(pp + i * 32 + lane);
     v[i] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
-    s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
   }
-  const float mean = warp_sum(s) * (1.0f / D);
-  float ss = 0.f;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
-    ss += (a * a + b * b) + (c * c + d * d);
-  }
-  const float rstd = rsqrtf(warp_sum(ss) * (1.0f / D) + 1e-8f);
+  float mean, rstd;
+  ln_row_stats<D>(v, 1e-8f, mean, rstd);
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const float4 g = __ldg(reinterpret_cast<const float4*>(gamma) + i * 32 + lane);
     const float4 b = __ldg(reinterpret_cast<const float4*>(beta) + i * 32 + lane);
-    float4 o = make_float4((v[i].x - mean) * rstd * g.x + b.x, (v[i].y - mean) * rstd * g.y + b.y,
-                           (v[i].z - mean) * rstd * g.z + b.z, (v[i].w - mean) * rstd * g.w + b.w);
-    reinterpret_cast<float4*>(out_f32 + static_cast<long long>(row) * D)[i * 32 + lane] = o;
-    if (split3) {
-      uint2 hi, lo;
-      pack_split2(o.x, o.y, hi.x, lo.x);
-      pack_split2(o.z, o.w, hi.y, lo.y);
-      uint2* dst = reinterpret_cast<uint2*>(out_bf16 + static_cast<long long>(row) * 3 * D) + i * 32 + lane;
-      dst[0] = hi; dst[D / 4] = lo; dst[D / 2] = hi;
-    } else {
-      uint2 pk;
-      pk.x = pack_bf16(o.x, o.y);
-      pk.y = pack_bf16(o.z, o.w);
-      reinterpret_cast<uint2*>(out_bf16 + static_cast<long long>(row) * D)[i * 32 + lane] = pk;
-    }
+    const float4 o = ln_norm(v[i], mean, rstd, g, b);
+    ln_store<D>(out_f32, out_bf16, split3, row, i * 32 + lane, o);
   }
   chain_signal(chain);
 }
@@ -464,41 +450,20 @@ embed_ln_rows_kernel(const long long* __restrict__ tokens, int T, const float* _
   const float4* wp = reinterpret_cast<const float4*>(words + tok * D);
   const float4* pp = reinterpret_cast<const float4*>(positions + static_cast<long long>(pos) * D);
   float4 v[NV];
-  float s = 0.f;
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const float4 a = __ldg(wp + i * 32 + lane);
     const float4 b = __ldg(pp + i * 32 + lane);
     v[i] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
-    s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
   }
-  const float mean = warp_sum(s) * (1.0f / D);
-  float ss = 0.f;
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
-    ss += (a * a + b * b) + (c * c + d * d);
-  }
-  const float rstd = rsqrtf(warp_sum(ss) * (1.0f / D) + 1e-8f);
+  float mean, rstd;
+  ln_row_stats<D>(v, 1e-8f, mean, rstd);
 #pragma unroll
   for (int i = 0; i < NV; ++i) {
     const float4 g = __ldg(reinterpret_cast<const float4*>(gamma) + i * 32 + lane);
     const float4 b = __ldg(reinterpret_cast<const float4*>(beta) + i * 32 + lane);
-    float4 o = make_float4((v[i].x - mean) * rstd * g.x + b.x, (v[i].y - mean) * rstd * g.y + b.y,
-                           (v[i].z - mean) * rstd * g.z + b.z, (v[i].w - mean) * rstd * g.w + b.w);
-    reinterpret_cast<float4*>(out_f32 + static_cast<long long>(row) * D)[i * 32 + lane] = o;
-    if (split3) {
-      uint2 hi, lo;
-      pack_split2(o.x, o.y, hi.x, lo.x);
-      pack_split2(o.z, o.w, hi.y, lo.y);
-      uint2* dst = reinterpret_cast<uint2*>(out_bf16 + static_cast<long long>(row) * 3 * D) + i * 32 + lane;
-      dst[0] = hi; dst[D / 4] = lo; dst[D / 2] = hi;
-    } else {
-      uint2 pk;
-      pk.x = pack_bf16(o.x, o.y);
-      pk.y = pack_bf16(o.z, o.w);
-      reinterpret_cast<uint2*>(out_bf16 + static_cast<long long>(row) * D)[i * 32 + lane] = pk;
-    }
+    const float4 o = ln_norm(v[i], mean, rstd, g, b);
+    ln_store<D>(out_f32, out_bf16, split3, row, i * 32 + lane, o);
   }
 }
 

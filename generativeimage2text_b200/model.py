@@ -335,7 +335,7 @@ class GitB200CaptioningModel(nn.Module):
             _lib.check(lib.gitb200_create(ctypes.byref(self._cfg), dev.index or 0, ctypes.byref(h)), None, 'create')
             sl['engine'], sl['sig'], sl['trie_key'] = h, None, None
             import os
-            for opt in ('use_graph', 'use_pdl', 'use_chain', 'use_mega', 'mega_coop', 'debug_layers', 'parity'):
+            for opt in ('use_graph', 'use_pdl', 'use_mega', 'debug_layers', 'parity'):
                 v = os.environ.get('GITB200_' + opt.upper())      # debugging switches, e.g. GITB200_USE_MEGA=0
                 if v is not None:
                     _lib.check(lib.gitb200_set_option(h, opt.encode(), int(v)), h, 'set_option')
@@ -381,7 +381,7 @@ class GitB200CaptioningModel(nn.Module):
             pass
 
     def set_engine_option(self, name, value):
-        """Engine switches (0/1): 'use_graph', 'use_pdl', 'use_chain', 'use_mega' (persistent one-kernel decode
+        """Engine switches (0/1): 'use_graph', 'use_pdl', 'use_mega' (persistent one-kernel decode
         step for greedy batches of <= 64), and 'parity' -- the fp32-grade
         verification mode (every GEMM as a three-term bf16 split product through the same wgmma kernels, fp32
         attention and K/V caches): logits within 1e-3 of the fp32 reference at ~3x the GEMM work."""

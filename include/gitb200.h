@@ -201,8 +201,8 @@ int gitb200_set_sampling(gitb200_engine* h, const float* uniforms_dev, int steps
 /* Number of kernels the engine launched since creation (bench.py's gpu_launches). */
 int64_t gitb200_launch_count(const gitb200_engine* h);
 /* Engine switches (defaults in parentheses): use_graph (1) CUDA-graph replay of the decode step, use_pdl (1) programmatic
- * dependent launch inside the step, use_chain (1) flag-ordered decode chain,
- * use_mega (1) greedy decode steps of <= 64 sequences as one persistent kernel (mega_coop (1): launched cooperatively),
+ * dependent launch inside the step (greedy steps on the kernel chain are then ordered by a flag chain),
+ * use_mega (1) greedy decode steps of <= 64 sequences as one persistent, cooperatively launched kernel,
  * parity (0) fp32-grade verification mode: every GEMM operand is a (hi, lo) bf16 pair and each product is computed as
  * a_hi w_hi + a_lo w_hi + a_hi w_lo by the same wgmma kernel (three K-segments side by side), attention / K/V caches /
  * q, k, v in fp32 -- set it BEFORE gitb200_set_weight (switching it forgets the uploaded weights). */

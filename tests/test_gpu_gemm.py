@@ -365,44 +365,44 @@ def _inst_id(p):
 # instantiations are in INSTANTIATIONS and the (hi, lo) arithmetic in test_parity_operands.
 ENGINE_CALLS = {
     # encode_impl: patch embedding, rows land at token 1 + patch of each image
-    'patch_b16_1img': ('g:1118', 196, 768, 768, dict(map=(196, 197, 1))),
-    'patch_b16_2img': ('g:1118', 2 * 196, 768, 768, dict(map=(196, 197, 1))),
-    'patch_b16_64img': ('g:1118', 64 * 196, 768, 768, dict(map=(196, 197, 1))),
-    'patch_l14_1img': ('g:1118', 256, 1024, 640, dict(map=(256, 257, 1))),          # K = 588 padded to 640
-    'patch_l14_2img': ('g:1118', 2 * 256, 1024, 640, dict(map=(256, 257, 1))),
-    'patch_l14_64img': ('g:1118', 64 * 256, 1024, 640, dict(map=(256, 257, 1))),
-    'patch_video_2x6': ('g:1118', 12 * 196, 768, 768, dict(map=(196, 197, 1))),      # 2 clips x 6 frames
-    'patch_ragged_lmax141': ('g:1118', 3 * 140, 768, 768, dict(map=(140, 141, 1))),  # every image owns L_max - 1 rows
-    'patch_ragged_tiny': ('g:1118', 40 * 3, 768, 768, dict(map=(3, 4, 1))),          # a 32-row block spans 11 images
+    'patch_b16_1img': ('g:1214', 196, 768, 768, dict(map=(196, 197, 1))),
+    'patch_b16_2img': ('g:1214', 2 * 196, 768, 768, dict(map=(196, 197, 1))),
+    'patch_b16_64img': ('g:1214', 64 * 196, 768, 768, dict(map=(196, 197, 1))),
+    'patch_l14_1img': ('g:1214', 256, 1024, 640, dict(map=(256, 257, 1))),          # K = 588 padded to 640
+    'patch_l14_2img': ('g:1214', 2 * 256, 1024, 640, dict(map=(256, 257, 1))),
+    'patch_l14_64img': ('g:1214', 64 * 256, 1024, 640, dict(map=(256, 257, 1))),
+    'patch_video_2x6': ('g:1214', 12 * 196, 768, 768, dict(map=(196, 197, 1))),      # 2 clips x 6 frames
+    'patch_ragged_lmax141': ('g:1214', 3 * 140, 768, 768, dict(map=(140, 141, 1))),  # every image owns L_max - 1 rows
+    'patch_ragged_tiny': ('g:1214', 40 * 3, 768, 768, dict(map=(3, 4, 1))),          # a 32-row block spans 11 images
     # encode_impl: the encoder layers
-    'enc_qkv_768': ('g:1139', 2 * 197, 2304, 768, dict(bias=True, out_bf16=True)),
-    'enc_qkv_1024': ('g:1139', 2 * 257, 3072, 1024, dict(bias=True, out_bf16=True)),
-    'enc_outproj_768': ('g:1158', 2 * 197, 768, 768, dict(bias=True, resid='inplace')),
-    'enc_outproj_1024': ('g:1158', 2 * 257, 1024, 1024, dict(bias=True, resid='inplace')),
-    'enc_cfc_768': ('g:1164', 2 * 197, 3072, 768, dict(bias=True, act=1, out_bf16=True)),
-    'enc_cfc_1024': ('g:1164', 2 * 257, 4096, 1024, dict(bias=True, act=1, out_bf16=True)),
-    'enc_cproj_768': ('g:1166', 2 * 197, 768, 3072, dict(bias=True, resid='inplace')),
-    'enc_cproj_1024': ('g:1166', 2 * 257, 1024, 4096, dict(bias=True, resid='inplace')),
-    'enc_cproj_768_64img': ('g:1166', 64 * 197 + 5, 768, 3072, dict(bias=True, resid='inplace')),
-    # prefill_impl
-    'visual_projection_768': ('g:1278', 2 * 197, 768, 768, dict(bias=True)),
-    'visual_projection_1024': ('g:1278', 2 * 257, 768, 1024, dict(bias=True)),
-    'prefill_qkv': ('g:1288', 2 * 197, 2304, 768, dict(bias=True, out_bf16=True, segs=3)),   # q scratch | K cache | V cache
-    'prefill_qkv_row_map': ('g:1288', 2 * 197, 2304, 768, dict(bias=True, out_bf16=True, segs=3, map=(197, 200, 2))),
-    'prefill_outproj': ('g:1306', 2 * 197, 768, 768, dict(bias=True, resid='other')),
-    'prefill_fc1': ('g:1311', 2 * 197, 3072, 768, dict(bias=True, act=2, out_bf16=True)),
-    'prefill_fc2': ('g:1313', 2 * 197, 768, 3072, dict(bias=True, resid='other')),
-    # score_impl (the LM head at e:751 is the statistics epilogue: test_lse_*)
-    'score_qkv': ('e:718', 5 * 13, 2304, 768, dict(bias=True, out_bf16=True, segs=3)),       # q | text K | text V
-    'score_qkv_parity': ('e:718', 5 * 13, 2304, 768, dict(bias=True, segs=3)),               # fp32 segments
-    'score_outproj': ('e:735', 5 * 13, 768, 768, dict(bias=True, resid='other')),
-    'score_fc1': ('e:740', 5 * 13, 3072, 768, dict(bias=True, act=2, out_bf16=True)),
-    'score_fc2': ('e:742', 5 * 13, 768, 3072, dict(bias=True, resid='other')),
+    'enc_qkv_768': ('g:1238', 2 * 197, 2304, 768, dict(bias=True, out_bf16=True)),
+    'enc_qkv_1024': ('g:1238', 2 * 257, 3072, 1024, dict(bias=True, out_bf16=True)),
+    'enc_outproj_768': ('g:1240', 2 * 197, 768, 768, dict(bias=True, resid='inplace')),
+    'enc_outproj_1024': ('g:1240', 2 * 257, 1024, 1024, dict(bias=True, resid='inplace')),
+    'enc_cfc_768': ('g:1242', 2 * 197, 3072, 768, dict(bias=True, act=1, out_bf16=True)),
+    'enc_cfc_1024': ('g:1242', 2 * 257, 4096, 1024, dict(bias=True, act=1, out_bf16=True)),
+    'enc_cproj_768': ('g:1243', 2 * 197, 768, 3072, dict(bias=True, resid='inplace')),
+    'enc_cproj_1024': ('g:1243', 2 * 257, 1024, 4096, dict(bias=True, resid='inplace')),
+    'enc_cproj_768_64img': ('g:1243', 64 * 197 + 5, 768, 3072, dict(bias=True, resid='inplace')),
+    # image_rows: the visual projection, then decoder_layers over the image rows
+    'visual_projection_768': ('g:1342', 2 * 197, 768, 768, dict(bias=True)),
+    'visual_projection_1024': ('g:1342', 2 * 257, 768, 1024, dict(bias=True)),
+    'prefill_qkv': ('g:1321', 2 * 197, 2304, 768, dict(bias=True, out_bf16=True, segs=3)),   # q scratch | K cache | V cache
+    'prefill_qkv_row_map': ('g:1321', 2 * 197, 2304, 768, dict(bias=True, out_bf16=True, segs=3, map=(197, 200, 2))),
+    'prefill_outproj': ('g:1324', 2 * 197, 768, 768, dict(bias=True, resid='other')),
+    'prefill_fc1': ('g:1326', 2 * 197, 3072, 768, dict(bias=True, act=2, out_bf16=True)),
+    'prefill_fc2': ('g:1327', 2 * 197, 768, 3072, dict(bias=True, resid='other')),
+    # score_impl: decoder_layers over the caption text rows (the LM head at e:696 is the statistics epilogue: test_lse_*)
+    'score_qkv': ('g:1321', 5 * 13, 2304, 768, dict(bias=True, out_bf16=True, segs=3)),       # q | text K | text V
+    'score_qkv_parity': ('g:1321', 5 * 13, 2304, 768, dict(bias=True, segs=3)),               # fp32 segments
+    'score_outproj': ('g:1324', 5 * 13, 768, 768, dict(bias=True, resid='other')),
+    'score_fc1': ('g:1326', 5 * 13, 3072, 768, dict(bias=True, act=2, out_bf16=True)),
+    'score_fc2': ('g:1327', 5 * 13, 768, 3072, dict(bias=True, resid='other')),
 }
-# Sites not in the table: step_layers' skinny calls (g:1357, DECODE_CALLS), the LM-head statistics (e:751, test_lse_*) and the
-# two hooks themselves (gitb200_op_gemm e:812, which tests/test_gpu_kernels.py runs, and gitb200_op_gemm_ex e:868).
-OTHER_SITES = ('g:1357', 'e:751', 'e:812', 'e:868')
-# step_layers' skinny calls (g:1357 through the `skinny` lambda): name -> (features, K, requested splits, bias, act, bf16)
+# Sites not in the table: step_layers' skinny calls (g:1434, DECODE_CALLS), the LM-head statistics (e:696, test_lse_*) and the
+# two hooks themselves (gitb200_op_gemm e:757, which tests/test_gpu_kernels.py runs, and gitb200_op_gemm_ex e:813).
+OTHER_SITES = ('g:1434', 'e:696', 'e:757', 'e:813')
+# step_layers' skinny calls (g:1434 through the `skinny` lambda): name -> (features, K, requested splits, bias, act, bf16)
 DECODE_CALLS = {
     'decode_qkv': (2304, 768, 3, False, 0, False),        # kQkvSplits
     'decode_outproj': (768, 768, 6, False, 0, False),     # kOutProjSplits
@@ -1122,12 +1122,12 @@ def test_lse_ownership_covers_every_column_once(N):
     assert torch.allclose(lse_fold_ref(ref), torch.logsumexp(x, 1), rtol=1e-12)
 
 
-def test_every_launch_gemm_call_site_is_named():
+def test_every_engine_gemm_call_site_is_named():
     """A new launch_gemm( call in the engine needs a case here: the sites named above are as many as the source has."""
     root = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'generativeimage2text_b200', 'csrc')
     calls = sum(open(os.path.join(root, f)).read().count('launch_gemm(h, ') for f in ('gitb200.cu', 'engine_api.inc'))
     named = {v[0] for v in ENGINE_CALLS.values()} | set(OTHER_SITES)
-    assert calls == len(named) == 18
+    assert calls == len(named) == 14
 
 
 def test_split_ranges_and_stages():

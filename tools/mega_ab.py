@@ -21,7 +21,7 @@ with torch.cuda.stream(s):
     for rows in rows_list:
         img = synthetic_images(rows).cuda()
         ref = None
-        for opts in ({'use_mega': 1, 'mega_coop': 1}, {'use_mega': 1, 'mega_coop': 0}, {'use_mega': 0}, {'use_mega': 1, 'mega_coop': 1}):
+        for opts in ({'use_mega': 1}, {'use_mega': 0}, {'use_mega': 1}):
             for k, v in opts.items():
                 m.set_engine_option(k, v)
             for _ in range(2):
