@@ -156,6 +156,7 @@ struct gitb200_engine {
 
   // workspaces
   DevBuf x, h, qkv, ctx, u, feats, feats_f32, pos_interp;   // encoder
+  int pos_rows = 0;                                         // rows of pos_interp the last encode re-sampled (0: none)
   DevBuf pt, pxd, phd, pq, pctx, pu;                        // decoder-layer pass (image rows, caption rows)
   DevBuf img_kv, txt_kv, src_row[2];                        // caches
   size_t txt_kv_eb = 0;                                     // element size (kvb()) the text cache was last zeroed for
@@ -1149,6 +1150,7 @@ static int ragged_setup(gitb200_engine* h, const std::vector<int>& hw, int B, in
   CK(cudaMemcpyAsync(h->rg_tab.p, tab.data(), static_cast<size_t>(B) * sizeof(RaggedImg), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(h->rg_lens.p, lens.data(), static_cast<size_t>(B) * 4, cudaMemcpyHostToDevice, st));
   h->cur_lens.swap(lens);
+  h->pos_rows = rows;
   *L_max = Lm;
   return 0;
 }
@@ -1167,6 +1169,7 @@ static int encode_impl(gitb200_engine* h, const float* images, int B, int frames
     frames = h->cfg.num_frames_emb;
   }
   h->cur_ragged = false;
+  h->pos_rows = 0;
   int L = h->Lc;
   if (rg) TRY(ragged_setup(h, ragged_hw, B, &L, st));
   const int d = h->d, gh = h->gh, gw = h->gw, Kp = h->Kp, H = h->cfg.enc_heads;
@@ -1198,6 +1201,7 @@ static int encode_impl(gitb200_engine* h, const float* images, int B, int frames
     pos_embed_bicubic_kernel<<<grid, 256, 0, st>>>(h->pos_emb.as<float>(), h->pos_interp.as<float>(), h->g, gh, gw, d);
     CKL(h, "pos_embed_bicubic_kernel");
     pos = h->pos_interp.as<float>();
+    h->pos_rows = L;
   }
   // patch embedding: im2col + GEMM, rows land at token index 1 + patch (CLS row is filled by the next kernel)
   // (ragged batches: every image owns L_max - 1 patch rows, the ones past its own grid are zero)

@@ -338,8 +338,15 @@ int gitb200_preproc_coeffs(int in_size, int out_size, int32_t* ksize_out, int32_
 /* Debug: copies one decode-step work buffer of the engine ("x", "y" fp32 [rows,768]; "hb", "ctx", "qb" bf16 [rows,768];
  * "ub" bf16 [rows,3072]) or cache ("img_kv": the image K/V [layer][k|v][image][token][768] of the last prefill, batch x
  * tokens rows; "txt_kv": the text K/V [layer][k|v][row][T_alloc][768], T_alloc = bytes / (layers * 2 * rows * 768 * element
- * size); both bf16, fp32 in parity mode) to host memory after a device synchronise.  Beam search bookkeeping, current
- * side of each ping-pong:
+ * size); both bf16, fp32 in parity mode) to host memory after a device synchronise.  The last encode (test hooks):
+ *   "enc_x"       fp32 [batch*frames*L][width]: the encoder's residual stream after its last block, before ln_post, images
+ *                 in the encoder's order f*batch + b (L: tokens per image; a ragged batch's slot length L_max);
+ *   "enc_feats"   the features as the prefill's GEMM operand: bf16 [batch*frames*L][width], or [hi | lo | hi] rows of
+ *                 3*width in parity mode (hi = bf16(f), lo = bf16(f - hi)); rows in the output order b*frames*L + f*L + l;
+ *   "pos_interp"  fp32 [rows][width]: the positional table the encode re-sampled, 1 + gh*gw rows for one input size, one
+ *                 table per distinct patch grid of a ragged batch in order of first appearance (the model's own grid copied);
+ *                 0 bytes when the encode used the stored table.
+ * Beam search bookkeeping, current side of each ping-pong:
  *   "src_row"     int32 [rows][T_alloc]: the text-K/V indirection table the next beam step reads (position j of logical
  *                 row r is held by physical row src_row[r][j]); after a beam generate or the raw decode_step API;
  *   "beam_ids"    int64 [rows][max_steps]: the token history (input_ids) of each beam, after a beam generate;

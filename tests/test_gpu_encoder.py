@@ -1,0 +1,574 @@
+"""Hot path A -- the image encoder (encode_impl) and the image rows of the prefill (image_rows) -- against the fp64
+statement of tests/encode_ref.py, stage by stage, in every input layout.
+
+Every stage is compared from the engine's OWN input to it, so each stage is measured on its own:
+  * the positional table the encode re-sampled ("pos_interp") against the fp64 bicubic re-sampling;
+  * engines built through the C ABI with 0, 1 and 2 encoder blocks (gitb200_create takes any enc_layers): the depth-0
+    residual stream ("enc_x") is the stem ln_pre(cls | patch + pos); block j is the depth-(j+1) stream against block j of
+    the depth-j stream.  This rests on identical launches on identical inputs giving identical results, which
+    test_depth_engines_are_deterministic asserts;
+  * ln_post (frame remap, temporal embeddings) from the engine's own stream, and the features' GEMM-operand copy
+    ("enc_feats") exactly;
+  * on the full-depth model: the visual projection from the engine's own operand copy, and the image K/V cache of all six
+    decoder layers from the engine's own projection (layer 0 alone, layers 1-5 as a chain), and the whole encoder
+    against the fp64 chain from the pixels (accumulation over 12 or 24 blocks).
+Default mode is compared with the bf16-rounding reference, parity mode with the pure fp64 one.  The same comparison with
+one defect planted in the reference must move the compared quantity by >= SENSITIVITY x its tolerance.
+
+Exact invariants: pixels the patch grid drops (a trailing partial patch) cannot change the features, even as NaN; the
+padding rows of a ragged batch are finite (zero in the stem); a tensor input and a one-frame list input give the same
+encoder stream, and features that differ by the temporal embedding only.
+"""
+import ctypes
+
+import pytest
+import torch
+
+import encode_ref as er
+from decode_ref import RefWeights, bf16
+
+# Largest |engine - reference| per mode and compared quantity: about 2x the largest error observed over these cases on
+# an H100 80GB HBM3 (132 SMs, 700 W power limit), given after each.  Default mode: the bf16 quantities (the image K/V)
+# differ from the reference by whole bf16 steps where the two round a value near a rounding boundary to neighbouring
+# bf16 numbers (0.0156 = one step at magnitudes 2 .. 4); the fp32 stages are compared from the engine's own bf16
+# operands, so only fp32 accumulation is left in them.
+TOL = {
+    'default': dict(pos=3.5e-7,    # 1.67e-7: positional table re-sampled (480x640)
+                    stem=7e-6,     # 3.47e-6: ln_pre(cls | patch + pos) (VATEX, 7 frames)
+                    block=0.0045,  # 0.00223: one ViT block (16x320)
+                    ln_post=2e-6,  # 1.00e-6: ln_post + temporal embedding, frame layout (VATEX, 7 frames)
+                    vproj=7.5e-6,  # 3.72e-6: visual projection + LN (L/14)
+                    kv0=0.016,     # 0.00781: decoder layer 0's image K / V, bf16
+                    kv=0.032,      # 0.0156: decoder layers 1-5's image K / V, bf16, chained from the engine's projection
+                    full=0.024),   # 0.0116: the whole encoder from the pixels (L/14, 24 blocks)
+    'parity': dict(pos=3.5e-7,     # 1.67e-7 (480x640)
+                   stem=5.2e-5,    # 2.58e-5 (VATEX, 7 frames)
+                   block=6.2e-5,   # 3.07e-5 (VATEX, 7 frames)
+                   ln_post=2.1e-6,  # 1.03e-6 (480x640)
+                   vproj=4.8e-5,   # 2.37e-5 (ragged)
+                   kv0=4.7e-5,     # 2.34e-5 (VATEX, 2 x 3 frames)
+                   kv=9.6e-5,      # 4.77e-5 (L/14)
+                   full=1.8e-4),   # 9.02e-5 (L/14)
+}
+SENSITIVITY = 4.0           # a planted defect must move a compared quantity by this many tolerances
+# At 1201 keys (480x640) a 64-key block holds ~5% of one head's weight and moves a default-mode block output by about
+# 1.3x its tolerance (0.0059 measured), so there the defect is only reported.  At 257 keys and fewer it clears 5x.
+LONG_ATTENTION = 1000
+
+MEASURED = {'default': {}, 'parity': {}}
+SENS = {}
+
+
+@pytest.fixture(scope='module', autouse=True)
+def _report_measured_errors():
+    """After the module: the largest error seen per mode and quantity, next to its tolerance (run pytest with -s)."""
+    yield
+    for mode in ('default', 'parity'):
+        for name, (e, case) in sorted(MEASURED[mode].items()):
+            print('DMAX %s %s %.3g (tolerance %.3g; %s)' % (mode, name, e, TOL[mode][name], case))
+    for key, (r, moved) in sorted(SENS.items()):
+        print('DSENS %s %.1f (moved %.3g)' % (key, r, moved))
+    for e in list(_ENGINES.values()):
+        _lib().gitb200_destroy(e.h)
+    _ENGINES.clear()
+
+
+def _track(mode, name, err, case):
+    if err > MEASURED[mode].get(name, (-1.0, ''))[0]:
+        MEASURED[mode][name] = (err, case)
+    assert err <= TOL[mode][name], (case, mode, name, err, TOL[mode][name])
+
+
+def _sens(mode, case, name, defect, moved, report_only=False):
+    """A planted defect moved a compared quantity by `moved`: it must be >= SENSITIVITY tolerances."""
+    r = moved / TOL[mode][name]
+    SENS['%s %s %s %s' % (case, mode, name, defect)] = (r, moved)
+    assert report_only or r >= SENSITIVITY, (case, mode, name, defect, r)
+
+
+def _err(a, b):
+    return (a.double() - b.double()).abs().max().item()
+
+
+class Tok:
+    cls_token_id, sep_token_id = 101, 102
+
+
+def _lib():
+    from generativeimage2text_b200 import _lib as L
+    return L.load()
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# CPU checks of the reference itself
+# ---------------------------------------------------------------------------------------------------------------------
+VATEX = {'num_image_with_embedding': 6}
+
+
+@pytest.fixture(scope='module')
+def sd_vatex():
+    from generativeimage2text_b200.synthetic import synthetic_state_dict
+    return synthetic_state_dict(VATEX, 1, 'perturbed')
+
+
+def _ref_encode(W, frames_px, list_input, n_blocks=None):
+    """The reference features of a list of frames [B, 3, H, W] (or one tensor input)."""
+    px = torch.cat(frames_px, dim=0)
+    B = frames_px[0].shape[0]
+    gh, gw = px.shape[2] // W.patch, px.shape[3] // W.patch
+    x = er.stem(W, px, er.resample_pos(W.pos, gh, gw))
+    for i in range(W.n_layers if n_blocks is None else n_blocks):
+        x = er.block(W, i, x)
+    return er.ln_post(W, x, B, len(frames_px), list_input)
+
+
+def test_encode_ref_without_rounding_is_the_oracle(sd_vatex):
+    """With rounding off, the stages chained are git_oracle's encode_image / visual_features / project_visual and the
+    image K/V of git_oracle.CachedDecoder, all run in fp64: re-sampled grid (48 x 80: 3 x 5 patches), 7 frames truncated
+    to the 6 temporal embeddings, and a tensor input without them."""
+    import git_oracle
+    sd64 = {k: v.double() for k, v in sd_vatex.items()}
+    W = er.EncWeights(sd_vatex, VATEX, rounding=False)
+    RW = RefWeights(sd_vatex, rounding=False)
+    g = torch.Generator().manual_seed(4)
+    frames = [torch.randn(2, 3, 48, 80, generator=g, dtype=torch.float64) for _ in range(7)]
+    want = git_oracle.visual_features(sd64, VATEX, frames)
+    got = _ref_encode(W, frames[:6], True)
+    assert got.shape == want.shape == (2, 6 * 16, 768)
+    assert (got - want).abs().max().item() <= 1e-9
+    want_t = git_oracle.visual_features(sd64, VATEX, frames[0])
+    got_t = _ref_encode(W, frames[:1], False)
+    assert (got_t - want_t).abs().max().item() <= 1e-9
+    v = er.vproj(W, got)
+    assert (v - git_oracle.project_visual(sd64, want)).abs().max().item() <= 1e-9
+    dec = git_oracle.CachedDecoder(sd64, want)
+    layers = er.image_layers(RW, v)
+    for j in range(6):
+        assert (layers[j]['k'] - dec.img_k[j]).abs().max().item() <= 1e-9
+        assert (layers[j]['v'] - dec.img_v[j]).abs().max().item() <= 1e-9
+
+
+def test_encode_ref_defects_are_planted_where_named(sd_vatex):
+    """Each planted defect changes the stage output where it is named and nowhere else."""
+    W = er.EncWeights(sd_vatex, VATEX, rounding=True, n_blocks=1)
+    g = torch.Generator().manual_seed(6)
+    same = torch.equal
+    # re-sampling: grid rows move, the class row does not; the A = -0.5 defect differs from F.interpolate in A alone
+    base = er.resample_pos(W.pos, 3, 5)
+    grid = W.pos[1:].reshape(14, 14, -1)
+    a075 = torch.einsum('yi,ijd,xj->yxd', er._cubic_matrix(14, 3, -0.75, False, grid.dtype, 'cpu'), grid,
+                        er._cubic_matrix(14, 5, -0.75, False, grid.dtype, 'cpu'))
+    assert (a075.reshape(15, -1) - base[1:]).abs().max().item() <= 1e-12
+    for defect in (('bicubic_a05',), ('align_corners',)):
+        d = er.resample_pos(W.pos, 3, 5, defect)
+        assert same(d[0], base[0]) and not same(d[1:], base[1:]), defect
+    # stem: the patch transpose moves the patch rows only, the missing pos[0] the class row only
+    px = torch.randn(2, 3, 48, 80, generator=g, dtype=torch.float64)
+    base = er.stem(W, px, er.resample_pos(W.pos, 3, 5))
+    d = er.stem(W, px, er.resample_pos(W.pos, 3, 5), ('patch_kxky',))
+    assert same(d[:, 0], base[:, 0]) and not same(d[:, 1:], base[:, 1:])
+    d = er.stem(W, px, er.resample_pos(W.pos, 3, 5), ('cls_nopos',))
+    assert not same(d[:, 0], base[:, 0]) and same(d[:, 1:], base[:, 1:])
+    # block: a key block already masked by an image's length changes nothing of that image; fc1 tile moves every row
+    x = torch.randn(2, 101, 768, generator=g, dtype=torch.float64)
+    lens = [101, 64]
+    base = er.block(W, 0, x, lens)
+    d = er.block(W, 0, x, lens, ('attn_keys', 3, 1))
+    assert not same(d[0], base[0]) and same(d[1, :64], base[1, :64])
+    d = er.block(W, 0, x, lens, ('fc1_tile', 5))
+    assert not (d[:, :64] == base[:, :64]).all(-1).any()
+    # ln_post: frames 0 / 1 swapped leave frame 2 alone; temb[0] everywhere leaves frame 0 alone
+    xf = torch.randn(3 * 2, 5, 768, generator=g, dtype=torch.float64)
+    base = er.ln_post(W, xf, 2, 3, True)
+    d = er.ln_post(W, xf, 2, 3, True, ('frames_swapped',))
+    assert not same(d[:, :10], base[:, :10]) and same(d[:, 10:], base[:, 10:])
+    d = er.ln_post(W, xf, 2, 3, True, ('temb0',))
+    assert same(d[:, :5], base[:, :5]) and not same(d[:, 5:], base[:, 5:])
+    assert same(er.ln_post(W, xf, 2, 3, False), er.ln_post(W, xf, 2, 3, False, ('temb0',)))
+    # visual projection, and the image layers: layer j's K moves, its V and the layers before it do not
+    f = bf16(torch.randn(2, 7, 768, generator=g))
+    assert not same(er.vproj(W, f, ('vproj_nobias',)), er.vproj(W, f))
+    RW = RefWeights(sd_vatex)
+    v = er.vproj(W, f)
+    base = er.image_layers(RW, v)
+    d = er.image_layers(RW, v, defect=('k_from_prev', 3))
+    for j in range(3):
+        assert same(d[j]['k'], base[j]['k']) and same(d[j]['v'], base[j]['v'])
+    assert not same(d[3]['k'], base[3]['k']) and same(d[3]['v'], base[3]['v'])
+    # parity mode: one operand rounded to bf16 moves the stage
+    Wp = er.EncWeights(sd_vatex, VATEX, rounding=False, n_blocks=1)
+    assert not same(er.stem(Wp, px, Wp.pos[:16], ('operand',)), er.stem(Wp, px, Wp.pos[:16]))
+    assert not same(er.block(Wp, 0, x, None, ('operand',)), er.block(Wp, 0, x))
+
+
+def test_feats_operand_split():
+    """hi + lo carries an fp32 value to within 2^-16 of itself; hi alone is its bf16 rounding."""
+    g = torch.Generator().manual_seed(9)
+    f = torch.randn(64, 768, generator=g)
+    op = er.feats_operand(f, True)
+    hi, lo, hi2 = op.split(768, dim=-1)
+    assert torch.equal(hi, hi2) and torch.equal(hi, er.feats_operand(f, False))
+    assert ((hi + lo - f.double()).abs() <= f.double().abs() * 2.0 ** -16).all()
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# GPU plumbing: engines of a given encoder depth through the C ABI
+# ---------------------------------------------------------------------------------------------------------------------
+FAMILIES = {
+    'b16': {},
+    'l14': {'image_encoder_type': 'CLIPViT_L_14', 'visual_feature_size': 1024},
+    'b16c160': {'test_crop_size': 160},
+    'vatex': VATEX,
+}
+_SD, _CFG, _REFW, _ENGINES = {}, {}, {}, {}
+
+
+def _sd(fam):
+    if fam not in _SD:
+        from generativeimage2text_b200.synthetic import synthetic_state_dict
+        _SD[fam] = synthetic_state_dict(FAMILIES[fam], 1, 'perturbed')
+    return _SD[fam]
+
+
+def _cfg(fam):
+    if fam not in _CFG:
+        from generativeimage2text_b200.model import get_git_model
+        _CFG[fam] = get_git_model(Tok(), FAMILIES[fam])._cfg
+    return _CFG[fam]
+
+
+def _refw(fam, mode):
+    key = (fam, mode)
+    if key not in _REFW:
+        rnd = mode == 'default'
+        _REFW[key] = (er.EncWeights(_sd(fam), FAMILIES[fam], rounding=rnd).to('cuda'),
+                      RefWeights(_sd(fam), rounding=rnd).to('cuda'))
+    return _REFW[key]
+
+
+class Engine(object):
+    """A C-ABI engine of the family's configuration with `depth` encoder blocks (None: all of them)."""
+
+    def __init__(self, fam, depth, parity):
+        from generativeimage2text_b200 import _lib as L
+        lib = L.load()
+        cfg = L.Config.from_buffer_copy(_cfg(fam))
+        if depth is not None:
+            cfg.enc_layers = depth
+        self.d, self.patch, self.n_emb = cfg.enc_width, cfg.patch, cfg.num_frames_emb
+        self.h = ctypes.c_void_p()
+        L.check(lib.gitb200_create(ctypes.byref(cfg), 0, ctypes.byref(self.h)), None, 'create')
+        L.check(lib.gitb200_set_option(self.h, b'parity', int(parity)), self.h, 'set_option')
+        for key, t in _sd(fam).items():
+            if key.startswith('image_encoder.transformer.resblocks.') and int(key.split('.')[3]) >= cfg.enc_layers:
+                continue
+            t = t.cuda().float().contiguous()
+            shape = (ctypes.c_int64 * t.dim())(*t.shape)
+            L.check(lib.gitb200_set_weight(self.h, key.encode(), t.data_ptr(), shape, t.dim(), L.F32, None), self.h,
+                    'set_weight')
+        L.check(lib.gitb200_finalize_weights(self.h, None), self.h, 'finalize_weights')
+
+    def encode(self, px, frames=0, sizes=None):
+        """px: [B, 3, H, W] (frames = 0: a tensor input), [frames, B, 3, H, W] (a list input) or, with sizes, the ragged
+        images back to back.  Returns feats_out [B, tokens, d]."""
+        from generativeimage2text_b200 import _lib as L
+        lib = L.load()
+        px = px.cuda().float().contiguous()
+        if sizes is not None:
+            B = len(sizes)
+            hw = (ctypes.c_int32 * (2 * B))(*[v for s in sizes for v in s])
+            L.check(lib.gitb200_set_image_sizes(self.h, hw, B), self.h, 'set_image_sizes')
+            p = self.patch
+            tokens = max((h // p) * (w // p) + 1 for h, w in sizes)
+        else:
+            B, H, W = px.shape[-4], px.shape[-2], px.shape[-1]
+            L.check(lib.gitb200_set_input_size(self.h, H, W), self.h, 'set_input_size')
+            p = self.patch
+            nf = min(frames, self.n_emb) if (frames and self.n_emb) else max(frames, 1)
+            tokens = nf * ((H // p) * (W // p) + 1)
+        self.B = B
+        out = torch.full((B, tokens, self.d), float('nan'), device='cuda')
+        L.check(lib.gitb200_encode(self.h, px.data_ptr(), B, frames, out.data_ptr(), None), self.h, 'encode')
+        torch.cuda.synchronize()
+        return out
+
+    def prefill(self, M):
+        from generativeimage2text_b200 import _lib as L
+        out = torch.full((self.B, M, 768), float('nan'), device='cuda')
+        L.check(L.load().gitb200_prefill(self.h, self.B, 1, out.data_ptr(), None), self.h, 'prefill')
+        torch.cuda.synchronize()
+        return out
+
+    def read(self, name, dtype):
+        buf = torch.empty(1 << 31, dtype=torch.uint8)
+        n = _lib().gitb200_debug_read(self.h, name.encode(), buf.data_ptr(), buf.numel())
+        assert n >= 0, 'debug_read(%s) failed' % name
+        return buf[:n].view(dtype).clone()
+
+
+def _engine(fam, depth, mode):
+    key = (fam, depth, mode)
+    if key not in _ENGINES:
+        _ENGINES[key] = Engine(fam, depth, mode == 'parity')
+    return _ENGINES[key]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# The case matrix
+# ---------------------------------------------------------------------------------------------------------------------
+# (id, family, input) -- input: dict(hw, B, frames) for one size, or dict(sizes) for a ragged batch.  prefill: the case
+# also runs the full-depth model's prefill; full: and compares the whole encoder with the fp64 chain.
+CASES = [
+    ('b16_224', 'b16', dict(hw=(224, 224), B=2), dict(prefill=True, full=True)),
+    ('l14_224', 'l14', dict(hw=(224, 224), B=2), dict(prefill=True, full=True)),
+    ('b16_crop160', 'b16c160', dict(hw=(160, 160), B=2), {}),
+    ('b16_480x640', 'b16', dict(hw=(480, 640), B=2), {}),
+    ('b16_230x250', 'b16', dict(hw=(230, 250), B=2), {}),
+    ('b16_16x320', 'b16', dict(hw=(16, 320), B=3), {}),
+    ('ragged', 'b16', dict(sizes=[(480, 640), (224, 224), (160, 224), (230, 250), (160, 224)]), dict(prefill=True)),
+    ('vatex_b2_f3', 'vatex', dict(hw=(224, 224), B=2, frames=3), dict(prefill=True)),
+    ('vatex_f7', 'vatex', dict(hw=(224, 224), B=2, frames=7), {}),
+    ('vatex_f0', 'vatex', dict(hw=(224, 224), B=2, frames=0), {}),
+]
+MODES = ['default', 'parity']
+
+
+def _pixels(inp, seed, fill=0.0):
+    """(engine input, reference images [N, 3, H, W] per image in the encoder's order) for a case.  Pixels of a trailing
+    partial patch are set to `fill` in both."""
+    g = torch.Generator().manual_seed(seed)
+    if 'sizes' in inp:
+        ims = [torch.randn(3, h, w, generator=g) for h, w in inp['sizes']]
+        for im in ims:
+            _fill_dropped(im, fill)
+        return torch.cat([im.reshape(-1) for im in ims]), [im[None] for im in ims]
+    H, W = inp['hw']
+    nf = max(inp.get('frames', 0), 1)
+    px = torch.randn(nf, inp['B'], 3, H, W, generator=g)
+    _fill_dropped(px, fill)
+    return (px if inp.get('frames', 0) else px[0]), px.reshape(nf * inp['B'], 3, H, W)
+
+
+def _fill_dropped(t, fill):
+    """The pixels past the last whole 16-pixel patch (the B/16 cases; every L/14 case is a multiple of 14)."""
+    H, W = t.shape[-2], t.shape[-1]
+    t[..., (H // 16) * 16:, :] = fill
+    t[..., :, (W // 16) * 16:] = fill
+
+
+def _geometry(fam, inp):
+    """(B, frames the engine keeps, list input, per-image (gh, gw), slot length L)."""
+    p = 14 if fam == 'l14' else 16
+    if 'sizes' in inp:
+        grids = [(h // p, w // p) for h, w in inp['sizes']]
+        return len(grids), 1, False, grids, max(a * b + 1 for a, b in grids)
+    frames = inp.get('frames', 0)
+    nf = min(max(frames, 1), 6) if fam == 'vatex' else max(frames, 1)
+    gh, gw = inp['hw'][0] // p, inp['hw'][1] // p
+    return inp['B'], nf, frames > 0, [(gh, gw)] * (inp['B'] * nf), gh * gw + 1
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('mode', MODES)
+@pytest.mark.parametrize('case', CASES, ids=[c[0] for c in CASES])
+def test_encoder_stages_against_fp64_reference(case, mode):
+    label, fam, inp, what = case
+    W, RW = _refw(fam, mode)
+    B, nf, list_input, grids, L = _geometry(fam, inp)
+    ragged = 'sizes' in inp
+    lens = [a * b + 1 for a, b in grids]
+    NI = B * nf
+    x_in, ref_px = _pixels(inp, 100 + len(label))
+    ref_px = [p.cuda().double() for p in ref_px] if ragged else ref_px[:NI].cuda().double()
+    frames_arg = inp.get('frames', 0)
+    sizes = inp.get('sizes')
+    tol = TOL[mode]
+
+    # 1. the positional tables of the distinct grids, in order of first appearance
+    e0 = _engine(fam, 0, mode)
+    x0_feats = e0.encode(x_in, frames_arg, sizes)
+    distinct = []
+    for gr in grids:
+        if gr not in distinct:
+            distinct.append(gr)
+    g0 = W.g0
+    pos_tabs = {gr: er.resample_pos(W.pos, *gr) for gr in distinct}
+    if ragged or distinct != [(g0, g0)]:
+        got = e0.read('pos_interp', torch.float32).reshape(-1, W.d).cuda()
+        want = torch.cat([pos_tabs[gr] for gr in distinct])
+        assert got.shape == want.shape
+        _track(mode, 'pos', _err(got, want), label)
+        for defect in (('bicubic_a05',), ('align_corners',)):
+            moved = max(_err(er.resample_pos(W.pos, *gr, defect), pos_tabs[gr]) for gr in distinct if gr != (g0, g0))
+            _sens(mode, label, 'pos', defect[0], moved)
+
+    # 2. depth 0: the stem
+    def stream(e):
+        return e.read('enc_x', torch.float32).reshape(NI, L, W.d).cuda()
+
+    def per_image(fn):
+        """fn(image index, its valid rows) -> [1, L_i, d]; returns the rows stacked into [NI, L, d] (NaN past L_i)."""
+        out = torch.full((NI, L, W.d), float('nan'), dtype=torch.float64, device='cuda')
+        for i in range(NI):
+            out[i, :lens[i]] = fn(i)[0, :lens[i]]
+        return out
+
+    def valid_err(a, b):
+        return max(_err(a[i, :lens[i]], b[i, :lens[i]]) for i in range(NI))
+
+    x0 = stream(e0)
+    if ragged:
+        for i in range(NI):
+            assert (x0[i, lens[i]:] == 0).all(), 'stem padding rows of image %d are not zero' % i
+
+        def stem_ref(defect=None):
+            return per_image(lambda i: er.stem(W, ref_px[i], pos_tabs[grids[i]], defect))
+    else:
+        def stem_ref(defect=None):
+            return er.stem(W, ref_px, pos_tabs[grids[0]], defect)
+    s_ref = stem_ref()
+    _track(mode, 'stem', valid_err(x0, s_ref), label)
+    stem_defects = [('patch_kxky',), ('cls_nopos',)] + ([('operand',)] if mode == 'parity' else [])
+    for defect in stem_defects:
+        _sens(mode, label, 'stem', defect[0], valid_err(stem_ref(defect), s_ref))
+
+    # 3. blocks 0 and 1, each from the engine's own stream of one block less
+    e1 = _engine(fam, 1, mode)
+    e1.encode(x_in, frames_arg, sizes)
+    x1 = stream(e1)
+    e2 = _engine(fam, 2, mode)
+    f2 = e2.encode(x_in, frames_arg, sizes)
+    x2 = stream(e2)
+    blens = lens if ragged else None
+    for j, (xin, xout) in enumerate(((x0, x1), (x1, x2))):
+        b_ref = er.block(W, j, xin.double(), blens)
+        _track(mode, 'block', valid_err(xout, b_ref), label)
+        if ragged:
+            assert torch.isfinite(xout).all(), 'block %d padding rows are not finite' % j
+        if j == 0:
+            defects = [('fc1_tile', 7)] + ([('attn_keys', 0, 1)] if min(lens) > 64 else [])
+            if mode == 'parity':
+                defects.append(('operand',))
+            for defect in defects:
+                moved = valid_err(er.block(W, j, xin.double(), blens, defect), b_ref)
+                _sens(mode, label, 'block', defect[0], moved, defect[0] == 'attn_keys' and max(lens) > LONG_ATTENTION)
+
+    # 4. ln_post from the engine's own stream; the operand copy exactly
+    if ragged:
+        f_ref = er.ln_post(W, x2.double(), B, 1, False)
+        ln_err = max(_err(f2[b, :lens[b]], f_ref[b, :lens[b]]) for b in range(B))
+        assert torch.isfinite(f2).all(), 'feature padding rows are not finite'
+    else:
+        f_ref = er.ln_post(W, x2.double(), B, nf, list_input)
+        ln_err = _err(f2, f_ref)
+    _track(mode, 'ln_post', ln_err, label)
+    if nf >= 2:
+        for defect in (('frames_swapped',), ('temb0',)):
+            _sens(mode, label, 'ln_post', defect[0], _err(er.ln_post(W, x2.double(), B, nf, list_input, defect), f_ref))
+    ops = e2.read('enc_feats', torch.bfloat16).reshape(B * f2.shape[1], -1).cuda()
+    assert torch.equal(ops.double(), er.feats_operand(f2.reshape(-1, W.d), mode == 'parity')), 'enc_feats'
+
+    # 5. / 6. the full-depth model: prefill stages and the whole encoder
+    if what.get('prefill') or what.get('full'):
+        ef = _engine(fam, None, mode)
+        feats = ef.encode(x_in, frames_arg, sizes)
+        if what.get('full'):
+            xx = s_ref
+            for i in range(W.n_layers):
+                xx = er.block(W, i, xx, blens)
+            full_ref = er.ln_post(W, xx, B, nf, list_input)
+            _track(mode, 'full', _err(feats, full_ref), label)
+        if what.get('prefill'):
+            M = feats.shape[1]
+            ops = ef.read('enc_feats', torch.bfloat16).reshape(B, M, -1).cuda().double()
+            fval = ops if mode == 'default' else ops[..., :W.d] + ops[..., W.d:2 * W.d]
+            vp = ef.prefill(M)
+            v_ref = er.vproj(W, fval)
+            if ragged:
+                assert torch.isfinite(vp).all()
+                vp_err = max(_err(vp[b, :lens[b]], v_ref[b, :lens[b]]) for b in range(B))
+                vp_moved = max(_err(er.vproj(W, fval, ('vproj_nobias',))[b, :lens[b]], v_ref[b, :lens[b]]) for b in range(B))
+            else:
+                vp_err = _err(vp, v_ref)
+                vp_moved = _err(er.vproj(W, fval, ('vproj_nobias',)), v_ref)
+            _track(mode, 'vproj', vp_err, label)
+            _sens(mode, label, 'vproj', 'vproj_nobias', vp_moved)
+            kv = ef.read('img_kv', torch.bfloat16 if mode == 'default' else torch.float32)
+            kv = kv.reshape(6, 2, B, M, 768).cuda()
+            if ragged:
+                assert torch.isfinite(kv).all(), 'image K/V padding rows are not finite'
+            klens = lens if ragged else None
+            ref_layers = er.image_layers(RW, vp.double(), klens)
+
+            def kv_err(layers, j, which):
+                got, want = kv[j, 0 if which == 'k' else 1], layers[j][which]
+                if ragged:
+                    return max(_err(got[b, :lens[b]], want[b, :lens[b]]) for b in range(B))
+                return _err(got, want)
+            for j in range(6):
+                for which in ('k', 'v'):
+                    _track(mode, 'kv0' if j == 0 else 'kv', kv_err(ref_layers, j, which), label)
+            bad = er.image_layers(RW, vp.double(), klens, ('k_from_prev', 3))
+            moved = max(_err(bad[3]['k'][b, :lens[b]], ref_layers[3]['k'][b, :lens[b]]) for b in range(B)) if ragged \
+                else _err(bad[3]['k'], ref_layers[3]['k'])
+            _sens(mode, label, 'kv', 'k_from_prev', moved)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Exact checks
+# ---------------------------------------------------------------------------------------------------------------------
+@pytest.mark.gpu
+def test_depth_engines_are_deterministic():
+    """The stage isolation above rests on identical launches on identical inputs giving identical results: the depth-1
+    engine run twice gives a bit-identical stream, and a full-depth engine built through the C ABI gives bit-identical
+    features to the Python model's own engine."""
+    from generativeimage2text_b200.model import get_git_model
+    inp = dict(hw=(224, 224), B=2)
+    x_in, _ = _pixels(inp, 7)
+    e1 = _engine('b16', 1, 'default')
+    e1.encode(x_in)
+    a = e1.read('enc_x', torch.float32)
+    e1.encode(x_in)
+    assert torch.equal(a, e1.read('enc_x', torch.float32))
+    m = get_git_model(Tok(), {})
+    m.load_state_dict(_sd('b16'), strict=False)
+    m = m.cuda().eval()
+    want = m.encode_image(x_in.cuda())
+    torch.cuda.synchronize()
+    got = _engine('b16', None, 'default').encode(x_in)
+    assert torch.equal(got, want)
+    m.release()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('mode', MODES)
+@pytest.mark.parametrize('ragged', [False, True], ids=['230x250', 'ragged'])
+def test_dropped_pixels_cannot_matter(ragged, mode):
+    """Pixels of a trailing partial patch are never read: NaN there gives bit-identical features to zeros there."""
+    inp = dict(sizes=[(480, 640), (230, 250), (160, 224)]) if ragged else dict(hw=(230, 250), B=2)
+    e = _engine('b16', 2, mode)
+    sizes = inp.get('sizes')
+    zero, _ = _pixels(inp, 21, 0.0)
+    nan, _ = _pixels(inp, 21, float('nan'))
+    assert torch.isnan(nan).any()
+    a = e.encode(zero, 0, sizes)
+    b = e.encode(nan, 0, sizes)
+    assert torch.equal(a.nan_to_num(7.0), b.nan_to_num(7.0)) and torch.equal(a.isnan(), b.isnan())
+    assert torch.isfinite(b).all()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('mode', MODES)
+def test_tensor_input_and_one_frame_list(mode):
+    """A bare tensor and a one-frame list run the same encoder (bit-identical streams); only the list input gets
+    temb[0], after ln_post."""
+    W, _ = _refw('vatex', mode)
+    e = _engine('vatex', 2, mode)
+    x_in, _ = _pixels(dict(hw=(224, 224), B=2), 33)
+    ft = e.encode(x_in, 0)
+    xt = e.read('enc_x', torch.float32)
+    fl = e.encode(x_in[None], 1)
+    xl = e.read('enc_x', torch.float32)
+    assert torch.equal(xt, xl)
+    d = _err(fl - ft, W.temb[0].float().expand_as(ft))
+    _track(mode, 'ln_post', d, 'vatex_list_vs_tensor')
