@@ -13,7 +13,7 @@
 //     the oracle makes the same choice.  (top_k / top_p are accepted and ignored by that class: the filter call is
 //     commented out, :372.)
 // One CTA per row, 256 threads, two passes over the row's fp32 logits (L2 resident).  Used by the kernel-chain decode step
-// in place of greedy_select_kernel; bookkeeping (tokens_out, log-prob sum, next token, loop state) is the same.
+// in place of greedy_select_kernel; the bookkeeping (resolve_row / commit_row, rowops.cuh) is the same.
 #pragma once
 #include "ptx.cuh"
 #include "rowops.cuh"
@@ -70,10 +70,7 @@ __global__ void __launch_bounds__(256) constrained_select_kernel(const SelectPar
   const int step = st->step, cur_len = st->cur_len;
   const float* z = p.logits + static_cast<long long>(row) * p.V;
   const long long last = p.next_token[row];
-  const int own_prefix = (p.row_prefix != nullptr) ? p.row_prefix_lens[p.row0 + row] : 0;
-  const bool in_prefix = (p.row_prefix != nullptr) && cur_len < own_prefix;
-  const bool first = (p.row_prefix != nullptr) ? (cur_len == own_prefix) : (step == 0);   // the row's first real decision
-  const bool row_done = (!first) && (!in_prefix) && (last == p.eos);
+  const RowStep rs = row_step(p, row, step, cur_len, last);
   const bool sampling = q.uniforms != nullptr;
   const float it = sampling ? q.inv_temperature : 1.0f;
   if (p.step_logits != nullptr) {
@@ -83,7 +80,7 @@ __global__ void __launch_bounds__(256) constrained_select_kernel(const SelectPar
   // the row after the reference's masks: no-repeat scatter (:330 / trie :122), never at a row's first decision
   auto val = [&](int i) -> float {
     float v = __ldcg(z + i);
-    if (!first && i == static_cast<int>(last)) v = -10000.0f;
+    if (!rs.first && i == static_cast<int>(last)) v = -10000.0f;
     return v;
   };
   // thread t owns the contiguous indices [t * C, (t + 1) * C): the inverse-CDF lookup needs index order
@@ -122,7 +119,7 @@ __global__ void __launch_bounds__(256) constrained_select_kernel(const SelectPar
   long long tok = garg;
   float lp = -logf(sum1);                   // z[arg] - max - log(sum exp(z - max)) with z[arg] == max
   int next_node = -1;
-  if (sampling && !row_done && !in_prefix) {
+  if (sampling && !rs.done && !rs.in_prefix) {
     // inclusive scan of the 256 thread masses in thread order (warp scans + the 8 warp totals in order)
     float inc = sT;
 #pragma unroll
@@ -160,9 +157,9 @@ __global__ void __launch_bounds__(256) constrained_select_kernel(const SelectPar
     tok = pick;
     const float vz = val(pick);
     // log-prob of the draw: tempered log-softmax at the row's first decision, un-tempered afterwards (see the header)
-    lp = first ? ((vz - gmax) * it - logf(total)) : ((vz - gmax) - logf(sum1));
+    lp = rs.first ? ((vz - gmax) * it - logf(total)) : ((vz - gmax) - logf(sum1));
   }
-  if (q.trie_begin != nullptr && !row_done && !in_prefix) {
+  if (q.trie_begin != nullptr && !rs.done && !rs.in_prefix) {
     const int node = q.trie_cursor[p.row0 + row];
     const int e0 = q.trie_begin[node], e1 = q.trie_begin[node + 1];
     if (e1 > e0) {
@@ -192,40 +189,9 @@ __global__ void __launch_bounds__(256) constrained_select_kernel(const SelectPar
     }
   }
   if (tid != 0) return;
-  if (in_prefix) {   // still feeding this row's prefix: the next prefix token, nothing to score
-    tok = p.row_prefix[static_cast<long long>(p.row0 + row) * p.row_prefix_stride + cur_len];
-    lp = 0.f;
-  } else if (row_done) {  // one-hot EOS distribution (reference :347-351 / trie :134-138)
-    tok = p.eos;
-    lp = 0.f;
-  }
   if (next_node >= 0) q.trie_cursor[p.row0 + row] = next_node;
-  p.tokens_out[static_cast<long long>(row) * p.max_steps + cur_len] = tok;
-  p.logprob_sum[row] += lp;
-  long long nxt = tok;
-  if (p.forced != nullptr) nxt = p.forced[static_cast<long long>(row) * p.max_steps + cur_len];
-  p.next_token[row] = nxt;
-  if (nxt != p.eos) atomicAdd(&st->not_eos, 1);
-  __threadfence();
-  const unsigned int tr = atomicAdd(&st->ticket, 1u);
-  if (tr == static_cast<unsigned int>(p.rows) - 1) {  // last row of this step: advance the loop state
-    __threadfence();
-    const int not_eos = atomicAdd(&st->not_eos, 0);
-    st->ticket = 0;
-    st->not_eos = 0;
-    st->cur_len = cur_len + 1;
-    st->final_len = cur_len + 1;
-    st->pos = st->pos + 1;
-    st->step = step + 1;
-    if (not_eos == 0) {
-      st->finished = 1;
-      if (step == 0 && p.row_prefix == nullptr) st->empty_caption = 1;
-    }
-    if (cur_len + 1 >= p.max_steps) st->finished = 1;
-    if (p.chain.counters != nullptr)
-      for (int k = 0; k < 64; ++k) p.chain.counters[k] = 0;
-    __threadfence();
-  }
+  const RowChoice c = resolve_row(p, row, cur_len, rs, tok, lp);
+  commit_row(p, row, step, cur_len, c, p.chain.counters);
 }
 
 __global__ void trie_reset_kernel(int* cursor, int rows) {

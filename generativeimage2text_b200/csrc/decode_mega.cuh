@@ -17,7 +17,9 @@
 //     from L2 into mma.sync fragments;
 //   * weights are stationary per CTA: a GEMM phase gives CTA c a few 8-feature tiles over a 768-long reduction; the 8 warps
 //     split a tile 4 row tiles x 2 K halves.  The 288 q | k | v tiles go out two per CTA, three for the first 288 - 2G.  fc2 (K = 3072) is dealt as 4 k slices x 96 feature tiles over 128 CTAs, its
-//     four partial sums meet in slice order in the LayerNorm phase: no atomics anywhere, the step is bit-reproducible;
+//     four partial sums meet in slice order in the LayerNorm phase: no atomics anywhere, the step is bit-reproducible.  One
+//     schedule (mega_tiles) says which tiles a CTA owns, for the producer and the compute warps alike, and every GEMM phase
+//     runs through one routine (mega_gemm);
 //   * attention: the 64-key chunks of a CTA's (sequence, head) items are dealt round-robin to its 8 warps, online-softmax
 //     states in shared memory, fixed-order merge.
 // The skinny GEMMs and the 1-row attention are HBM-bound byte work (arithmetic intensity ~rows FLOP/B): they use the
@@ -43,8 +45,12 @@ constexpr int kMegaKvSubRows = 16;         // a chunk of fewer keys is fetched i
 constexpr int kMegaMaxRows = 64;
 constexpr int kMegaD = 768, kMegaF = 3072, kMegaH = 12;
 constexpr int kMegaAttItems = 6;           // (sequence, head) attention items of the busiest CTA: ceil(64 * 12 / 132)
-constexpr int kMegaMinCtas = 128;          // fc1 / fc2 deal their tiles over 128 CTAs; attention needs ceil(64 * 12 / G) <= 6
-constexpr int kMegaQkvTiles = 288;         // q | k | v: 2304 features in 8-feature tiles, 2-3 per CTA (needs G >= 96)
+constexpr int kMegaOutTiles = kMegaD / 8;  // 96 tiles of 8 output features: out-proj (one per CTA), fc2
+constexpr int kMegaQkvTiles = 3 * kMegaD / 8;                  // 288 q | k | v tiles, 2-3 per CTA (needs G >= 96)
+constexpr int kMegaFcTilesPerCta = 3;                          // fc1 / fc2 tiles per CTA
+constexpr int kMegaFcCtas = kMegaF / 8 / kMegaFcTilesPerCta;   // 128 CTAs take fc1's 384 tiles and fc2's 96 x 4 k slices
+constexpr int kMegaFc2Slices = kMegaF / kMegaD;                // fc2's 3072-long reduction as 4 slices of 768
+constexpr int kMegaMinCtas = kMegaFcCtas;  // attention also needs ceil(64 * 12 / G) <= 6
 constexpr int kMegaAttState = 72;          // floats per (item, warp) softmax state: 64 output dims, running max, 4 lane sums
 constexpr unsigned int kMegaSpinLimit = 1u << 18;   // bounded waits: a protocol bug must end in an error code, not a hung device
 
@@ -52,7 +58,7 @@ struct MegaLayer {
   const uint8_t* wqkv;     // [288] tiles: features 8t .. 8t+7 of the fused q | k | v projection
   const uint8_t* wo;       // [96]
   const uint8_t* w1;       // [384]
-  const uint8_t* w2;       // [96][4]: feature tile x 768-wide k slice (CTA c < 128: slice c & 3 of tiles 3 (c >> 2) .. + 2)
+  const uint8_t* w2;       // [96][4]: feature tile x 768-wide k slice (mega_w2_tile)
   const float* bqkv; const float* bo; const float* b1; const float* b2;
   const float* lnag; const float* lnab; const float* lnog; const float* lnob;
   __nv_bfloat16* txt_k;    // [R, T_alloc, 768]
@@ -66,7 +72,7 @@ struct MegaParams {
   const float* words;      // fp32 [V, 768] (embedding gather)
   const float* positions;  // fp32 [max_pos, 768]
   const float* lnemb_g; const float* lnemb_b;
-  int R, M, T_alloc, V, n_layers;
+  int M, T_alloc, n_layers;
   // activations (global, L2 resident)
   float* x;                // [R, 768] residual stream (post-LayerNorm)
   float* y;                // [R, 768] pre-LayerNorm sum (after the attention block)
@@ -75,15 +81,42 @@ struct MegaParams {
   __nv_bfloat16* qb;       // [R, 768] q (+bias) / 8
   __nv_bfloat16* ctx;      // [R, 768]
   __nv_bfloat16* ub;       // [R, 3072]
-  float* part_max; float* part_sum; int* part_arg;   // [R, gridDim.x] LM-head partials
-  // search state (the same objects greedy_select_kernel works on)
-  StepState* state;
-  long long* tokens_out; int max_steps; float* logprob_sum; long long* next_token; const long long* forced;
-  float* step_logits; int eos;
-  const long long* row_prefix; int row_prefix_stride; const int* row_prefix_lens;   // per-row prefixes (see SelectParams)
+  // the search state greedy_select_kernel works on (R = sel.rows, V = sel.V); the LM-head partials are [R, gridDim.x]
+  SelectParams sel;
   unsigned int* barrier;   // [2] grid-barrier counters, used alternately by successive steps
   int* error;              // set non-zero when a bounded spin gave up (the host reports it)
 };
+
+// ---- the tile schedule: what CTA `cta` of G owns in each GEMM phase ----------------------------------------------------
+// The producer walks it to fill the ring and the compute warps to take the ring's chunks in the same order; fc2's weights are
+// packed by mega_w2_tile to match.  (The attention chunks of a CTA are dealt in the kernel's prologue: round_keys.)
+enum MegaGemm { kGemmQkv, kGemmOut, kGemmFc1, kGemmFc2, kGemmLm };
+struct MegaTiles {
+  int t0, n, stride;   // tiles t0 + j * stride (j < n) of the phase's packed weight buffer
+  int f0;              // tile j computes output features 8 (f0 + j) .. 8 (f0 + j) + 7
+  int a_col;           // first column of the A operand (fc2: the CTA's k slice)
+};
+__device__ __forceinline__ int mega_lm_per(int V, int G) { return ((V + 7) / 8 + G - 1) / G; }
+// fc2's packed weights: the tile of features 8f .. 8f + 7 over k slice s (k = 768 s .. 768 s + 767)
+__host__ __device__ constexpr int mega_w2_tile(int f, int s) { return f * kMegaFc2Slices + s; }
+__device__ __forceinline__ MegaTiles mega_tiles(MegaGemm ph, int cta, int G, int V, int lm_per) {
+  if (ph == kGemmQkv) {   // one pass: two each, three for the first 288 - 2G CTAs when G < 144 (contiguous ranges)
+    const int extra = max(0, kMegaQkvTiles - 2 * G);
+    const int t0 = (cta < extra) ? 3 * cta : 2 * cta + extra;
+    return {t0, (cta < extra) ? 3 : max(0, min(2, kMegaQkvTiles - t0)), 1, t0, 0};
+  }
+  if (ph == kGemmOut) return {cta, cta < kMegaOutTiles ? 1 : 0, 1, cta, 0};
+  if (ph == kGemmFc1) {
+    const int t0 = cta * kMegaFcTilesPerCta;
+    return {t0, cta < kMegaFcCtas ? kMegaFcTilesPerCta : 0, 1, t0, 0};
+  }
+  if (ph == kGemmFc2) {   // feature group cta / 4 (3 tiles) x k slice cta % 4
+    const int f0 = (cta / kMegaFc2Slices) * kMegaFcTilesPerCta, ks = cta % kMegaFc2Slices;
+    return {mega_w2_tile(f0, ks), cta < kMegaFcCtas ? kMegaFcTilesPerCta : 0, mega_w2_tile(1, 0), f0, ks * kMegaD};
+  }
+  const int t0 = cta * lm_per;   // LM head: ceil(V / 8) tiles in contiguous ranges of lm_per = mega_lm_per(V, G)
+  return {t0, max(0, min(lm_per, (V + 7) / 8 - t0)), 1, t0, 0};
+}
 
 // ---- packing: [N, K] row-major bf16 -> tiles of 8 features x 768 k in fragment order ------------------------------------
 // Tile layout: 48 k-steps x 32 lanes x 8 bytes.  Lane (g = lane / 4, t = lane % 4) of k-step s holds the four k values
@@ -139,6 +172,8 @@ struct MegaTl {
   }
 };
 #define MEGA_TL(kid) tlf.mark(kid)
+// makes the next mark wait until the A operand's loads have landed
+#define MEGA_TL_DEP(a, error) if (((a).lo[5][7] ^ (a).hi[5][7] ^ (a).lo[0][0]) == 0x9E3779B9u) *(error) = kWaitTimelineProbe;
 #else
 struct MegaTl {
   __device__ __forceinline__ void begin() {}
@@ -146,6 +181,7 @@ struct MegaTl {
   __device__ __forceinline__ void end() {}
 };
 #define MEGA_TL(kid)
+#define MEGA_TL_DEP(a, error)
 #endif
 
 __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
@@ -171,14 +207,14 @@ struct MegaRing {
   volatile uint32_t* issued;   // chunks the producer has armed so far (shared memory)
   __device__ __forceinline__ const uint8_t* acquire() {
     const uint32_t slot = idx % kMegaSlots;
-    if (!mbar_wait_bounded(&full[slot], (idx / kMegaSlots) & 1, error)) *error = 2;
+    if (!mbar_wait_bounded(&full[slot], (idx / kMegaSlots) & 1, error)) *error = kWaitRingFull;
     return base + slot * kMegaSlotBytes;
   }
   // chunk idx + n (n < kMegaSlots) without consuming it: the GEMM phases take all tiles of a batch first, so that the MMAs
   // of one tile overlap the shared-memory reads, the K-half exchange and the epilogue of its neighbours
   __device__ __forceinline__ const uint8_t* acquire_ahead(uint32_t n) {
     const uint32_t i = idx + n, slot = i % kMegaSlots;
-    if (!mbar_wait_bounded(&full[slot], (i / kMegaSlots) & 1, error)) *error = 2;
+    if (!mbar_wait_bounded(&full[slot], (i / kMegaSlots) & 1, error)) *error = kWaitRingFull;
     return base + slot * kMegaSlotBytes;
   }
   __device__ __forceinline__ void release() {   // every compute warp, once per chunk
@@ -194,9 +230,9 @@ struct MegaRing {
     const uint32_t slot = i % kMegaSlots;
     unsigned int spins = 0;
     while (*issued <= i) {
-      if (++spins > (kMegaSpinLimit << 4) || ((spins & 1023u) == 1023u && *reinterpret_cast<const volatile int*>(error) != 0)) { *error = 5; break; }
+      if (++spins > (kMegaSpinLimit << 4) || ((spins & 1023u) == 1023u && *reinterpret_cast<const volatile int*>(error) != 0)) { *error = kWaitRingArmed; break; }
     }
-    if (!mbar_wait_bounded(&full[slot], (i / kMegaSlots) & 1, error)) *error = 2;
+    if (!mbar_wait_bounded(&full[slot], (i / kMegaSlots) & 1, error)) *error = kWaitRingFull;
     return base + slot * kMegaSlotBytes;
   }
   __device__ __forceinline__ void release_at(uint32_t i) {
@@ -223,7 +259,7 @@ __device__ __forceinline__ void mega_grid_sync(unsigned int* counter, unsigned i
     unsigned int spins = 0;
     while (ld_acquire_gpu(counter) < epoch) {
       if (++spins > kMegaSpinLimit || ((spins & 255u) == 255u && *reinterpret_cast<const volatile int*>(error) != 0)) {
-        if (*reinterpret_cast<const volatile int*>(error) == 0) *error = 1;
+        if (*reinterpret_cast<const volatile int*>(error) == 0) *error = kWaitGridBarrier;
         break;
       }
     }
@@ -338,6 +374,50 @@ __device__ __forceinline__ void mega_combine_both_n(float (&c)[NT][4], float4* r
   }
 }
 
+// Zeroes c, takes the next NT ring chunks (timeline mark tl_landed once they landed), runs the MMAs and frees the chunks.
+template <int NT>
+__device__ __forceinline__ void mega_ring_mma(float (&c)[NT][4], MegaRing& rg, const MegaAFrag& a, int kh, int lane, MegaTl& tlf,
+                                              int tl_landed) {
+  const uint8_t* tb[NT];
+#pragma unroll
+  for (int j = 0; j < NT; ++j) {
+    c[j][0] = c[j][1] = c[j][2] = c[j][3] = 0.f;
+    tb[j] = rg.acquire_ahead(j);
+  }
+  if (tl_landed) tlf.mark(tl_landed);
+  mega_mma_tiles<NT>(c, a, tb, kh, lane);
+#pragma unroll
+  for (int j = 0; j < NT; ++j) rg.release();
+}
+// One GEMM phase: the NT tiles s of this CTA (mega_tiles) against A[:rows, s.a_col ..) (leading dimension lda), plus bias
+// when kBias.  The epilogue epi(c, f, b) runs in the warp that owns tile j's sum: c[0..1] = row r0, c[2..3] = row r0 + 8
+// of output features f, f + 1, and b their bias (0 without one).  Timeline marks tl_id + 0 .. 4 (tl_id = 0: none).
+// kBias is a template argument, not a null test: a bias chosen at run time compiles to selects that make the warp wait
+// for the bias loads before its MMAs (in the timeline build the q | k | v and fc1 phases took ~2 us longer that way).
+template <int NT, bool kBias, class Epi>
+__device__ __forceinline__ void mega_gemm(MegaRing& rg, float4* red, int& red_buf, const __nv_bfloat16* A, long long lda, int rows,
+                                          const MegaTiles& s, const float* bias, int mt, int kh, int lane, MegaTl& tlf, int tl_id,
+                                          Epi&& epi) {
+  const int t = lane & 3;
+  MegaAFrag a;
+  if (tl_id) tlf.mark(tl_id + 0);
+  mega_load_a(a, A + s.a_col, lda, rows, mt, kh, lane);
+  if (tl_id) { tlf.mark(tl_id + 1); MEGA_TL_DEP(a, rg.error) tlf.mark(tl_id + 2); }
+  float2 bias_j[NT];
+#pragma unroll
+  for (int j = 0; j < NT; ++j)
+    bias_j[j] = kBias ? __ldg(reinterpret_cast<const float2*>(bias + (s.f0 + j) * 8 + 2 * t)) : make_float2(0.f, 0.f);
+  float c[NT][4];
+  mega_ring_mma<NT>(c, rg, a, kh, lane, tlf, tl_id ? tl_id + 3 : 0);
+  const bool own = mega_combine_n<NT>(c, red, red_buf, mt, kh, lane);
+  if (tl_id) tlf.mark(tl_id + 4);
+  if (own) {
+#pragma unroll
+    for (int j = 0; j < NT; ++j) epi(c[j], (s.f0 + j) * 8 + 2 * t, bias_j[j]);
+  }
+  red_buf ^= 1;
+}
+
 __device__ __forceinline__ float2 ldcg_f2(const float* p) { return __ldcg(reinterpret_cast<const float2*>(p)); }
 
 // ---- the kernel ----------------------------------------------------------------------------------------------------------
@@ -359,11 +439,11 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
   uint64_t* empty = full + kMegaSlots;
   volatile uint32_t* issued = reinterpret_cast<volatile uint32_t*>(empty + kMegaSlots);
 
-  StepState* st = p.state;
+  StepState* st = p.sel.state;
   if (st->finished) return;                     // stable: only the previous launch's selection phase writes it
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int cta = blockIdx.x, G = gridDim.x;
-  const int R = p.R, M = p.M;
+  const int R = p.sel.rows, M = p.M;
   const int pos = st->pos, step = st->step, cur_len = st->cur_len;
   const int n_kv = (M + kMegaKvRows - 1) / kMegaKvRows;
   const int n_txt = pos / 64 + 1;               // 64-position chunks of the text K/V cache holding positions 0 .. pos
@@ -373,14 +453,7 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
   const int n_items = R * kMegaH;
   const int my_cta_rev = G - 1 - cta;           // attention items are dealt from the last CTA down (those own fewer weights)
   const int n_my_items = (n_items > my_cta_rev) ? (n_items - my_cta_rev + G - 1) / G : 0;
-  const int lm_tiles_total = (p.V + 7) / 8;
-  const int lm_per = (lm_tiles_total + G - 1) / G;
-  const int lm_t0 = cta * lm_per;
-  const int lm_n = max(0, min(lm_per, lm_tiles_total - lm_t0));
-  // q | k | v tiles of this CTA, one pass: two each, three for the first 288 - 2G CTAs when G < 144 (contiguous ranges)
-  const int qkv_extra = max(0, kMegaQkvTiles - 2 * G);
-  const int qkv_t0 = (cta < qkv_extra) ? 3 * cta : 2 * cta + qkv_extra;
-  const int qkv_n = (cta < qkv_extra) ? 3 : max(0, min(2, kMegaQkvTiles - qkv_t0));
+  const int lm_per = mega_lm_per(p.sel.V, G);   // the GEMM phases' weight tiles of this CTA: mega_tiles
 
   if (tid == 0) {
     tma_prefetch_desc(&tmKV);
@@ -403,7 +476,7 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
       uint32_t i = 0;
       auto slot_ready = [&]() -> uint8_t* {
         const uint32_t slot = i % kMegaSlots;
-        if (i >= kMegaSlots && !mbar_wait_bounded(&empty[slot], ((i / kMegaSlots) - 1) & 1, p.error)) *p.error = 3;
+        if (i >= kMegaSlots && !mbar_wait_bounded(&empty[slot], ((i / kMegaSlots) - 1) & 1, p.error)) *p.error = kWaitRingEmpty;
         return ring + slot * kMegaSlotBytes;
       };
       auto publish = [&]() {          // the chunk's barrier is armed: consumers may now wait for its phase
@@ -411,11 +484,13 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
         __threadfence_block();
         *issued = i;
       };
-      auto tile = [&](const uint8_t* src) {
-        uint8_t* dst = slot_ready();
-        mbar_arrive_expect_tx(&full[i % kMegaSlots], kMegaTileBytes);
-        bulk_load_1d(dst, src, kMegaTileBytes, &full[i % kMegaSlots]);
-        publish();
+      auto tiles = [&](const uint8_t* w, const MegaTiles& s) {   // one GEMM phase's weight tiles
+        for (int j = 0; j < s.n; ++j) {
+          uint8_t* dst = slot_ready();
+          mbar_arrive_expect_tx(&full[i % kMegaSlots], kMegaTileBytes);
+          bulk_load_1d(dst, w + static_cast<size_t>(s.t0 + j * s.stride) * kMegaTileBytes, kMegaTileBytes, &full[i % kMegaSlots]);
+          publish();
+        }
       };
       // one attention chunk: up to 64 keys of one (sequence, head) with n valid, K rows at the slot's start, V rows 8 KB
       // in.  n = 64: one 64-row box each.  n < 64: ceil(n / 16) 16-row boxes each, sub-box s at byte 2048 s of its half --
@@ -444,7 +519,7 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
       };
       for (int l = 0; l < p.n_layers; ++l) {
         const MegaLayer& L = p.layer[l];
-        for (int j = 0; j < qkv_n; ++j) tile(L.wqkv + static_cast<size_t>(qkv_t0 + j) * kMegaTileBytes);
+        tiles(L.wqkv, mega_tiles(kGemmQkv, cta, G, p.sel.V, lm_per));
         // attention chunks ("units") of this CTA's items, round-major: unit u = r * n_my_items + k is keys 64r .. 64r + 63 of
         // item k (image keys first, then the text rounds), of which round_keys(r) are fetched; the consumer deals the
         // units to its 8 warps round-robin
@@ -456,7 +531,7 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
             unsigned int spins = 0;
             while (ld_acquire_gpu(p.barrier + (step & 1)) < target) {
               if (++spins > kMegaSpinLimit || ((spins & 255u) == 255u && *reinterpret_cast<const volatile int*>(p.error) != 0)) {
-                if (*reinterpret_cast<const volatile int*>(p.error) == 0) *p.error = 4;
+                if (*reinterpret_cast<const volatile int*>(p.error) == 0) *p.error = kWaitTextKv;
                 break;
               }
             }
@@ -473,11 +548,11 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
                       ((l * 2 + 1) * R + b) * p.T_alloc + (r - n_kv) * 64, h * 64, n_keys);
           }
         }
-        if (cta < 96) tile(L.wo + static_cast<size_t>(cta) * kMegaTileBytes);
-        if (cta < 128) for (int j = 0; j < 3; ++j) tile(L.w1 + static_cast<size_t>(cta * 3 + j) * kMegaTileBytes);
-        if (cta < 128) for (int j = 0; j < 3; ++j) tile(L.w2 + static_cast<size_t>(((cta >> 2) * 3 + j) * 4 + (cta & 3)) * kMegaTileBytes);
+        tiles(L.wo, mega_tiles(kGemmOut, cta, G, p.sel.V, lm_per));
+        tiles(L.w1, mega_tiles(kGemmFc1, cta, G, p.sel.V, lm_per));
+        tiles(L.w2, mega_tiles(kGemmFc2, cta, G, p.sel.V, lm_per));
       }
-      for (int j = 0; j < lm_n; ++j) tile(p.lm + static_cast<size_t>(lm_t0 + j) * kMegaTileBytes);
+      tiles(p.lm, mega_tiles(kGemmLm, cta, G, p.sel.V, lm_per));
     }
     return;
   }
@@ -490,10 +565,8 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
   tlf.begin();
 #ifdef GITB200_TIMELINE
 #define MEGA_TL_ID(ph) ((l == 2) ? 710000 + (ph) * 100 : 0)
-#define MEGA_TL_DEP(a) if (((a).lo[5][7] ^ (a).hi[5][7] ^ (a).lo[0][0]) == 0x9E3779B9u) *p.error = 99;
 #else
 #define MEGA_TL_ID(ph) 0
-#define MEGA_TL_DEP(a)
 #endif
   const int mt = warp & 3, kh = warp >> 2;
   const int g = lane >> 2, t = lane & 3;
@@ -503,52 +576,26 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
   for (int l = 0; l < p.n_layers; ++l) {
     const MegaLayer& L = p.layer[l];
     // ------------------------------------------------ P1: q | k | v ------------------------------------------------
-    auto qkv_tiles = [&](auto nt) {
-      constexpr int NT = decltype(nt)::value;
-      MegaAFrag a;
-      if (MEGA_TL_ID(1)) tlf.mark(MEGA_TL_ID(1) + 0);
-      mega_load_a(a, p.hb, kMegaD, R, mt, kh, lane);
-      if (MEGA_TL_ID(1)) { tlf.mark(MEGA_TL_ID(1) + 1); MEGA_TL_DEP(a) tlf.mark(MEGA_TL_ID(1) + 2); }
-      float2 bias_j[NT];
+    {
+      const MegaTiles s = mega_tiles(kGemmQkv, cta, G, p.sel.V, lm_per);
+      auto qkv_out = [&](const float (&c)[4], int f, float2 bias) {   // q / 8 | this position's text K | V
+        const int seg = f / kMegaD, fo = f - seg * kMegaD;
 #pragma unroll
-      for (int j = 0; j < NT; ++j) bias_j[j] = __ldg(reinterpret_cast<const float2*>(L.bqkv + (qkv_t0 + j) * 8 + 2 * t));
-      float c[NT][4];
-      const uint8_t* tb[NT];
-#pragma unroll
-      for (int j = 0; j < NT; ++j) {
-        c[j][0] = c[j][1] = c[j][2] = c[j][3] = 0.f;
-        tb[j] = rg.acquire_ahead(j);
-      }
-      if (MEGA_TL_ID(1)) tlf.mark(MEGA_TL_ID(1) + 3);
-      mega_mma_tiles<NT>(c, a, tb, kh, lane);
-#pragma unroll
-      for (int j = 0; j < NT; ++j) rg.release();
-      const bool own1 = mega_combine_n<NT>(c, redv, red_buf, mt, kh, lane);
-      if (MEGA_TL_ID(1)) tlf.mark(MEGA_TL_ID(1) + 4);
-      if (own1) {
-#pragma unroll
-        for (int j = 0; j < NT; ++j) {
-          const int f = (qkv_t0 + j) * 8 + 2 * t;
-          const float2 bias = bias_j[j];
-          const int seg = f / kMegaD, fo = f - seg * kMegaD;
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            const int r = hh ? r1 : r0;
-            if (r >= R) continue;
-            const float v0 = c[j][2 * hh] + bias.x, v1 = c[j][2 * hh + 1] + bias.y;
-            if (seg == 0) {
-              *reinterpret_cast<uint32_t*>(p.qb + static_cast<long long>(r) * kMegaD + fo) = pack_bf16(v0 * 0.125f, v1 * 0.125f);
-            } else {
-              __nv_bfloat16* dst = (seg == 1 ? L.txt_k : L.txt_v) + (static_cast<long long>(r) * p.T_alloc + pos) * kMegaD + fo;
-              *reinterpret_cast<uint32_t*>(dst) = pack_bf16(v0, v1);
-            }
+        for (int hh = 0; hh < 2; ++hh) {
+          const int r = hh ? r1 : r0;
+          if (r >= R) continue;
+          const float v0 = c[2 * hh] + bias.x, v1 = c[2 * hh + 1] + bias.y;
+          if (seg == 0) {
+            *reinterpret_cast<uint32_t*>(p.qb + static_cast<long long>(r) * kMegaD + fo) = pack_bf16(v0 * 0.125f, v1 * 0.125f);
+          } else {
+            __nv_bfloat16* dst = (seg == 1 ? L.txt_k : L.txt_v) + (static_cast<long long>(r) * p.T_alloc + pos) * kMegaD + fo;
+            *reinterpret_cast<uint32_t*>(dst) = pack_bf16(v0, v1);
           }
         }
-      }
-      red_buf ^= 1;
-    };
-    if (qkv_n == 3) qkv_tiles(std::integral_constant<int, 3>());
-    else if (qkv_n == 2) qkv_tiles(std::integral_constant<int, 2>());
+      };
+      if (s.n == 3) mega_gemm<3, true>(rg, redv, red_buf, p.hb, kMegaD, R, s, L.bqkv, mt, kh, lane, tlf, MEGA_TL_ID(1), qkv_out);
+      else if (s.n == 2) mega_gemm<2, true>(rg, redv, red_buf, p.hb, kMegaD, R, s, L.bqkv, mt, kh, lane, tlf, MEGA_TL_ID(1), qkv_out);
+    }
     mega_grid_sync(bar, epoch, p.error, tlf, MEGA_TL_ID(1));
     // ------------------------------------------------ P2: attention ------------------------------------------------
     // The CTA's 5-6 (sequence, head) items x (image + text) 64-key chunks form U units; warp w takes units w, w + 8, ...
@@ -706,28 +753,24 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
     }
     mega_grid_sync(bar, epoch, p.error, tlf, MEGA_TL_ID(2));
     // ------------------------------------------------ P3: attention output projection (+bias +residual) ------------------
-    if (cta < 96) {
-      MegaAFrag a;
-      mega_load_a(a, p.ctx, kMegaD, R, mt, kh, lane);
-      const int f = cta * 8 + 2 * t;
-      const float2 bias = __ldg(reinterpret_cast<const float2*>(L.bo + f));
-      float2 xr[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};      // residual: requested before the MMA needs the tile
-      if (kh == 0 && r0 < R) xr[0] = ldcg_f2(p.x + static_cast<long long>(r0) * kMegaD + f);
-      if (kh == 0 && r1 < R) xr[1] = ldcg_f2(p.x + static_cast<long long>(r1) * kMegaD + f);
-      float c[1][4] = {{0.f, 0.f, 0.f, 0.f}};
-      const uint8_t* tb[1] = {rg.acquire_ahead(0)};
-      mega_mma_tiles<1>(c, a, tb, kh, lane);
-      rg.release();
-      if (mega_combine_n<1>(c, redv, red_buf, mt, kh, lane)) {
+    {
+      const MegaTiles s = mega_tiles(kGemmOut, cta, G, p.sel.V, lm_per);
+      if (s.n > 0) {
+        const int f = s.f0 * 8 + 2 * t;
+        float2 xr[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};      // residual: requested before the MMA needs the tile
+        if (kh == 0 && r0 < R) xr[0] = ldcg_f2(p.x + static_cast<long long>(r0) * kMegaD + f);
+        if (kh == 0 && r1 < R) xr[1] = ldcg_f2(p.x + static_cast<long long>(r1) * kMegaD + f);
+        auto out_proj = [&](const float (&c)[4], int f, float2 bias) {
 #pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          const int r = hh ? r1 : r0;
-          if (r >= R) continue;
-          *reinterpret_cast<float2*>(p.y + static_cast<long long>(r) * kMegaD + f) =
-              make_float2(xr[hh].x + (c[0][2 * hh] + bias.x), xr[hh].y + (c[0][2 * hh + 1] + bias.y));
-        }
+          for (int hh = 0; hh < 2; ++hh) {
+            const int r = hh ? r1 : r0;
+            if (r >= R) continue;
+            *reinterpret_cast<float2*>(p.y + static_cast<long long>(r) * kMegaD + f) =
+                make_float2(xr[hh].x + (c[2 * hh] + bias.x), xr[hh].y + (c[2 * hh + 1] + bias.y));
+          }
+        };
+        mega_gemm<1, true>(rg, redv, red_buf, p.ctx, kMegaD, R, s, L.bo, mt, kh, lane, tlf, MEGA_TL_ID(3), out_proj);
       }
-      red_buf ^= 1;
     }
     mega_grid_sync(bar, epoch, p.error, tlf, MEGA_TL_ID(3));
     // ------------------------------------------------ P4 / P7: LayerNorm(y) -> x, hb (warp 0 of CTA r: row r) ----------------
@@ -760,98 +803,44 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
             v[i].w = xx[i].w + ((((q0[i].w + q1[i].w) + q2[i].w) + q3[i].w) + bb.w);
           }
         }
-        float s = 0.f;
-#pragma unroll
-        for (int i = 0; i < 6; ++i) s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
-        const float mean = warp_sum(s) * (1.0f / kMegaD);
-        float ss = 0.f;
-#pragma unroll
-        for (int i = 0; i < 6; ++i) {
-          const float a = v[i].x - mean, b2 = v[i].y - mean, c2 = v[i].z - mean, d2 = v[i].w - mean;
-          ss += (a * a + b2 * b2) + (c2 * c2 + d2 * d2);
-        }
-        const float rstd = rsqrtf(warp_sum(ss) * (1.0f / kMegaD) + 1e-12f);
+        float mean, rstd;
+        ln_row_stats<kMegaD>(v, 1e-12f, mean, rstd);
 #pragma unroll
         for (int i = 0; i < 6; ++i) {
           const float4 gm = __ldg(reinterpret_cast<const float4*>(gamma) + i * 32 + lane);
           const float4 bt = __ldg(reinterpret_cast<const float4*>(beta) + i * 32 + lane);
-          float4 ov;
-          ov.x = (v[i].x - mean) * rstd * gm.x + bt.x;
-          ov.y = (v[i].y - mean) * rstd * gm.y + bt.y;
-          ov.z = (v[i].z - mean) * rstd * gm.z + bt.z;
-          ov.w = (v[i].w - mean) * rstd * gm.w + bt.w;
-          reinterpret_cast<float4*>(p.x + static_cast<long long>(row) * kMegaD)[i * 32 + lane] = ov;
-          uint2 pk;
-          pk.x = pack_bf16(ov.x, ov.y);
-          pk.y = pack_bf16(ov.z, ov.w);
-          reinterpret_cast<uint2*>(p.hb + static_cast<long long>(row) * kMegaD)[i * 32 + lane] = pk;
+          ln_store<kMegaD>(p.x, p.hb, 0, row, i * 32 + lane, ln_norm(v[i], mean, rstd, gm, bt));
         }
       }
     };
     layer_norm_rows(L.lnag, L.lnab, false, nullptr);
     mega_grid_sync(bar, epoch, p.error, tlf, MEGA_TL_ID(4));
     // ------------------------------------------------ P5: fc1 + erf-GELU ------------------------------------------------
-    if (cta < 128) {
-      MegaAFrag a;
-      if (MEGA_TL_ID(5)) tlf.mark(MEGA_TL_ID(5) + 0);
-      mega_load_a(a, p.hb, kMegaD, R, mt, kh, lane);
-      if (MEGA_TL_ID(5)) { tlf.mark(MEGA_TL_ID(5) + 1); MEGA_TL_DEP(a) tlf.mark(MEGA_TL_ID(5) + 2); }
-      float2 bias_j[3];
+    {
+      const MegaTiles s = mega_tiles(kGemmFc1, cta, G, p.sel.V, lm_per);
+      auto fc1_out = [&](const float (&c)[4], int f, float2 bias) {
 #pragma unroll
-      for (int j = 0; j < 3; ++j) bias_j[j] = __ldg(reinterpret_cast<const float2*>(L.b1 + (cta * 3 + j) * 8 + 2 * t));
-      float c[3][4];
-#pragma unroll
-      for (int j = 0; j < 3; ++j) c[j][0] = c[j][1] = c[j][2] = c[j][3] = 0.f;
-      const uint8_t* tb[3] = {rg.acquire_ahead(0), rg.acquire_ahead(1), rg.acquire_ahead(2)};
-      if (MEGA_TL_ID(5)) tlf.mark(MEGA_TL_ID(5) + 3);
-      mega_mma_tiles<3>(c, a, tb, kh, lane);
-      rg.release();
-      rg.release();
-      rg.release();
-      const bool own5 = mega_combine_n<3>(c, redv, red_buf, mt, kh, lane);
-      if (MEGA_TL_ID(5)) tlf.mark(MEGA_TL_ID(5) + 4);
-      if (own5) {
-#pragma unroll
-        for (int j = 0; j < 3; ++j) {
-          const int f = (cta * 3 + j) * 8 + 2 * t;
-          const float2 bias = bias_j[j];
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            const int r = hh ? r1 : r0;
-            if (r >= R) continue;
-            *reinterpret_cast<uint32_t*>(p.ub + static_cast<long long>(r) * kMegaF + f) =
-                pack_bf16(apply_act(c[j][2 * hh] + bias.x, ACT_GELU_ERF), apply_act(c[j][2 * hh + 1] + bias.y, ACT_GELU_ERF));
-          }
+        for (int hh = 0; hh < 2; ++hh) {
+          const int r = hh ? r1 : r0;
+          if (r >= R) continue;
+          *reinterpret_cast<uint32_t*>(p.ub + static_cast<long long>(r) * kMegaF + f) =
+              pack_bf16(apply_act(c[2 * hh] + bias.x, ACT_GELU_ERF), apply_act(c[2 * hh + 1] + bias.y, ACT_GELU_ERF));
         }
-      }
-      red_buf ^= 1;
+      };
+      if (s.n > 0) mega_gemm<kMegaFcTilesPerCta, true>(rg, redv, red_buf, p.hb, kMegaD, R, s, L.b1, mt, kh, lane, tlf, MEGA_TL_ID(5), fc1_out);
     }
     mega_grid_sync(bar, epoch, p.error, tlf, MEGA_TL_ID(5));
     // ------------------------------------------------ P6: fc2, split over CTAs: 32 groups of 24 features x 4 k slices ------
     // (each CTA reads ONE 768-wide slice of the activations; the four partial sums of a feature meet, in slice order, in
     //  the LayerNorm phase below -- bit-reproducible, no atomics)
-    if (cta < 128) {
-      const int ks = cta & 3, fg = cta >> 2;
-      MegaAFrag a;
-      mega_load_a(a, p.ub + ks * kMegaD, kMegaF, R, mt, kh, lane);
-      float* yp = p.ypart + static_cast<long long>(ks) * R * kMegaD;
-      float c[3][4];
-#pragma unroll
-      for (int j = 0; j < 3; ++j) c[j][0] = c[j][1] = c[j][2] = c[j][3] = 0.f;
-      const uint8_t* tb[3] = {rg.acquire_ahead(0), rg.acquire_ahead(1), rg.acquire_ahead(2)};
-      mega_mma_tiles<3>(c, a, tb, kh, lane);
-      rg.release();
-      rg.release();
-      rg.release();
-      if (mega_combine_n<3>(c, redv, red_buf, mt, kh, lane)) {
-#pragma unroll
-        for (int j = 0; j < 3; ++j) {
-          const int f = (fg * 3 + j) * 8 + 2 * t;
-          if (r0 < R) *reinterpret_cast<float2*>(yp + static_cast<long long>(r0) * kMegaD + f) = make_float2(c[j][0], c[j][1]);
-          if (r1 < R) *reinterpret_cast<float2*>(yp + static_cast<long long>(r1) * kMegaD + f) = make_float2(c[j][2], c[j][3]);
-        }
-      }
-      red_buf ^= 1;
+    {
+      const MegaTiles s = mega_tiles(kGemmFc2, cta, G, p.sel.V, lm_per);
+      float* yp = p.ypart + static_cast<long long>(s.a_col) * R;     // the partial buffer of k slice a_col / 768
+      auto fc2_out = [&](const float (&c)[4], int f, float2) {
+        if (r0 < R) *reinterpret_cast<float2*>(yp + static_cast<long long>(r0) * kMegaD + f) = make_float2(c[0], c[1]);
+        if (r1 < R) *reinterpret_cast<float2*>(yp + static_cast<long long>(r1) * kMegaD + f) = make_float2(c[2], c[3]);
+      };
+      if (s.n > 0) mega_gemm<kMegaFcTilesPerCta, false>(rg, redv, red_buf, p.ub, kMegaF, R, s, nullptr, mt, kh, lane, tlf, MEGA_TL_ID(6), fc2_out);
     }
     mega_grid_sync(bar, epoch, p.error, tlf, MEGA_TL_ID(6));
     layer_norm_rows(L.lnog, L.lnob, true, L.b2);
@@ -863,35 +852,38 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
   // those of row g + 8: for its row and its 2 columns per tile a thread maintains the running (max, arg max, sum exp) over
   // this CTA's features -- the logits themselves never leave the SM (unless the parity hook asks for them).
   {
+    const MegaTiles lm = mega_tiles(kGemmLm, cta, G, p.sel.V, lm_per);
     const int my_row = kh ? r1 : r0;
     long long last = -1;
-    bool first = (step == 0);                       // no no-repeat mask at a row's first real decision
+    // no no-repeat mask at a row's first real decision, nor inside its prefix, whose token is given: row_step's first ||
+    // in_prefix, spelled out here because the row_step call spills registers in this kernel
+    bool unmasked = (step == 0);
     if (my_row < R) {
-      last = p.next_token[my_row];
-      if (p.row_prefix != nullptr) first = cur_len <= p.row_prefix_lens[my_row];
+      last = p.sel.next_token[my_row];
+      if (p.sel.row_prefix != nullptr) unmasked = cur_len <= p.sel.row_prefix_lens[my_row];
     }
     float smax = -INFINITY, ssum = 0.f;
     int sarg = 0x7fffffff;
     float* bias_s = att_part;                       // this CTA's slice of the output bias (<= 8 * lm_per floats)
-    for (int i = tid; i < lm_n * 8; i += kMegaComputeWarps * 32) {
-      const int col = lm_t0 * 8 + i;
-      bias_s[i] = (col < p.V) ? __ldg(p.lm_bias + col) : 0.f;
+    for (int i = tid; i < lm.n * 8; i += kMegaComputeWarps * 32) {
+      const int col = lm.t0 * 8 + i;
+      bias_s[i] = (col < p.sel.V) ? __ldg(p.lm_bias + col) : 0.f;
     }
     named_bar_sync(1, kMegaComputeWarps * 32);
-    if (lm_n > 0) {
+    if (lm.n > 0) {
       MegaAFrag a;
       mega_load_a(a, p.hb, kMegaD, R, mt, kh, lane);
       // statistics of one tile's two columns of this thread's row (columns arrive in increasing order)
       auto lm_stats = [&](const float (&cc)[4], int j) {
         if (my_row >= R) return;
-        const int f = (lm_t0 + j) * 8 + 2 * t;
+        const int f = (lm.t0 + j) * 8 + 2 * t;
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int col = f + e;
-          if (col >= p.V) continue;
+          if (col >= p.sel.V) continue;
           float v = (kh ? cc[2 + e] : cc[e]) + bias_s[j * 8 + 2 * t + e];
-          if (p.step_logits != nullptr) p.step_logits[(static_cast<long long>(step) * R + my_row) * p.V + col] = v;
-          if (!first && col == static_cast<int>(last)) v = -10000.0f;        // no-repeat (reference :330)
+          if (p.sel.step_logits != nullptr) p.sel.step_logits[(static_cast<long long>(step) * R + my_row) * p.sel.V + col] = v;
+          if (!unmasked && col == static_cast<int>(last)) v = -10000.0f;     // no-repeat (reference :330)
           if (v > smax) {            // the lowest index wins exact ties
             ssum = ssum * __expf(smax - v) + 1.0f;
             smax = v;
@@ -903,13 +895,9 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
       };
       int j = 0;
       MEGA_TL(720000);                                // LM head: A loads issued
-      for (; j + 2 <= lm_n; j += 2) {                 // two tiles in flight per warp (see mega_mma_tiles)
-        float c[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-        const uint8_t* tb[2] = {rg.acquire_ahead(0), rg.acquire_ahead(1)};
-        MEGA_TL(720100 + j);                          // the pair's tiles landed
-        mega_mma_tiles<2>(c, a, tb, kh, lane);
-        rg.release();
-        rg.release();
+      for (; j + 2 <= lm.n; j += 2) {                 // two tiles in flight per warp (see mega_mma_tiles)
+        float c[2][4];
+        mega_ring_mma<2>(c, rg, a, kh, lane, tlf, 720100 + j);   // mark: the pair's tiles landed
         mega_combine_both_n<2>(c, redv, red_buf, warp, mt, kh, lane);
         MEGA_TL(720200 + j);                          // MMAs + exchange done
         red_buf ^= 1;
@@ -917,11 +905,9 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
         lm_stats(c[1], j + 1);
         MEGA_TL(720300 + j);                          // statistics done
       }
-      if (j < lm_n) {
-        float c[1][4] = {{0.f, 0.f, 0.f, 0.f}};
-        const uint8_t* tb[1] = {rg.acquire_ahead(0)};
-        mega_mma_tiles<1>(c, a, tb, kh, lane);
-        rg.release();
+      if (j < lm.n) {
+        float c[1][4];
+        mega_ring_mma<1>(c, rg, a, kh, lane, tlf, 0);
         mega_combine_both_n<1>(c, redv, red_buf, warp, mt, kh, lane);
         red_buf ^= 1;
         lm_stats(c[0], j);
@@ -929,21 +915,13 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
     }
     // combine the 4 lanes of a quad (they hold the same row, interleaved column pairs)
 #pragma unroll
-    for (int o2 = 1; o2 <= 2; o2 <<= 1) {
-      const float m_o = __shfl_xor_sync(0xffffffffu, smax, o2);
-      const float s_o = __shfl_xor_sync(0xffffffffu, ssum, o2);
-      const int a_o = __shfl_xor_sync(0xffffffffu, sarg, o2);
-      const float mn = fmaxf(smax, m_o);
-      const float sa = (smax == -INFINITY) ? 0.f : __expf(smax - mn);
-      const float sb = (m_o == -INFINITY) ? 0.f : __expf(m_o - mn);
-      ssum = ssum * sa + s_o * sb;
-      if (m_o > smax || (m_o == smax && a_o < sarg)) sarg = a_o;
-      smax = mn;
-    }
+    for (int o2 = 1; o2 <= 2; o2 <<= 1)
+      merge_stats(smax, ssum, sarg, __shfl_xor_sync(0xffffffffu, smax, o2), __shfl_xor_sync(0xffffffffu, ssum, o2),
+                  __shfl_xor_sync(0xffffffffu, sarg, o2));
     if (t == 0 && my_row < R) {
-      p.part_max[static_cast<long long>(my_row) * G + cta] = smax;
-      p.part_sum[static_cast<long long>(my_row) * G + cta] = ssum;
-      p.part_arg[static_cast<long long>(my_row) * G + cta] = sarg;
+      p.sel.part_max[static_cast<long long>(my_row) * G + cta] = smax;
+      p.sel.part_sum[static_cast<long long>(my_row) * G + cta] = ssum;
+      p.sel.part_arg[static_cast<long long>(my_row) * G + cta] = sarg;
     }
   }
   mega_grid_sync(bar, epoch, p.error, tlf, 0);
@@ -952,106 +930,19 @@ decode_mega_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_consta
   // ------------------------------------------------ selection (greedy bookkeeping) + next token's embedding ----------------
   if (cta < R && warp == 0) {
     const int row = cta;
-    const int own_prefix = (p.row_prefix != nullptr) ? p.row_prefix_lens[row] : 0;
-    const bool in_prefix = (p.row_prefix != nullptr) && cur_len < own_prefix;
-    const bool first = (p.row_prefix != nullptr) ? (cur_len == own_prefix) : (step == 0);
     float gm = -INFINITY, gs = 0.f;
     int ga = 0x7fffffff;
-    for (int k = lane; k < G; k += 32) {           // increasing CTA order = increasing column order
-      const float pm = __ldcg(p.part_max + static_cast<long long>(row) * G + k);
-      const float ps = __ldcg(p.part_sum + static_cast<long long>(row) * G + k);
-      const int pa2 = __ldcg(p.part_arg + static_cast<long long>(row) * G + k);
-      const float mn = fmaxf(gm, pm);
-      const float sa = (gm == -INFINITY) ? 0.f : __expf(gm - mn);
-      const float sb = (pm == -INFINITY) ? 0.f : __expf(pm - mn);
-      gs = gs * sa + ps * sb;
-      if (pm > gm || (pm == gm && pa2 < ga)) ga = pa2;
-      gm = mn;
-    }
+    for (int k = lane; k < G; k += 32)             // increasing CTA order = increasing column order
+      merge_stats(gm, gs, ga, __ldcg(p.sel.part_max + static_cast<long long>(row) * G + k),
+                  __ldcg(p.sel.part_sum + static_cast<long long>(row) * G + k), __ldcg(p.sel.part_arg + static_cast<long long>(row) * G + k));
 #pragma unroll
-    for (int o2 = 16; o2 > 0; o2 >>= 1) {
-      const float m_o = __shfl_xor_sync(0xffffffffu, gm, o2);
-      const float s_o = __shfl_xor_sync(0xffffffffu, gs, o2);
-      const int a_o = __shfl_xor_sync(0xffffffffu, ga, o2);
-      const float mn = fmaxf(gm, m_o);
-      const float sa = (gm == -INFINITY) ? 0.f : __expf(gm - mn);
-      const float sb = (m_o == -INFINITY) ? 0.f : __expf(m_o - mn);
-      gs = gs * sa + s_o * sb;
-      if (m_o > gm || (m_o == gm && a_o < ga)) ga = a_o;
-      gm = mn;
-    }
-    const long long last = p.next_token[row];
-    const bool row_done = (!first) && (!in_prefix) && (last == p.eos);
-    long long tok = row_done ? p.eos : ga;                         // EOS forcing: one-hot distribution, log-prob 0
-    float lp = row_done ? 0.f : -logf(gs);
-    if (in_prefix) {                                               // still feeding this row's prefix
-      tok = p.row_prefix[static_cast<long long>(row) * p.row_prefix_stride + cur_len];
-      lp = 0.f;
-    }
-    long long nxt = tok;
-    if (p.forced != nullptr) nxt = p.forced[static_cast<long long>(row) * p.max_steps + cur_len];
-    if (lane == 0) {
-      p.tokens_out[static_cast<long long>(row) * p.max_steps + cur_len] = tok;
-      p.logprob_sum[row] += lp;
-      p.next_token[row] = nxt;
-    }
-    // embedding of the token the next step feeds: e = LN(words[nxt] + positions[pos + 1], eps 1e-8)
-    {
-      long long tk = nxt < 0 ? 0 : (nxt >= p.V ? p.V - 1 : nxt);
-      const float4* wp = reinterpret_cast<const float4*>(p.words + tk * kMegaD);
-      const float4* pp = reinterpret_cast<const float4*>(p.positions + static_cast<long long>(pos + 1) * kMegaD);
-      float4 v[6];
-      float s = 0.f;
-#pragma unroll
-      for (int i = 0; i < 6; ++i) {
-        const float4 a = __ldg(wp + i * 32 + lane);
-        const float4 b2 = __ldg(pp + i * 32 + lane);
-        v[i] = make_float4(a.x + b2.x, a.y + b2.y, a.z + b2.z, a.w + b2.w);
-        s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
-      }
-      const float mean = warp_sum(s) * (1.0f / kMegaD);
-      float ss = 0.f;
-#pragma unroll
-      for (int i = 0; i < 6; ++i) {
-        const float a = v[i].x - mean, b2 = v[i].y - mean, c2 = v[i].z - mean, d2 = v[i].w - mean;
-        ss += (a * a + b2 * b2) + (c2 * c2 + d2 * d2);
-      }
-      const float rstd = rsqrtf(warp_sum(ss) * (1.0f / kMegaD) + 1e-8f);
-#pragma unroll
-      for (int i = 0; i < 6; ++i) {
-        const float4 gmm = __ldg(reinterpret_cast<const float4*>(p.lnemb_g) + i * 32 + lane);
-        const float4 bt = __ldg(reinterpret_cast<const float4*>(p.lnemb_b) + i * 32 + lane);
-        float4 ov = make_float4((v[i].x - mean) * rstd * gmm.x + bt.x, (v[i].y - mean) * rstd * gmm.y + bt.y,
-                                (v[i].z - mean) * rstd * gmm.z + bt.z, (v[i].w - mean) * rstd * gmm.w + bt.w);
-        reinterpret_cast<float4*>(p.x + static_cast<long long>(row) * kMegaD)[i * 32 + lane] = ov;
-        uint2 pk;
-        pk.x = pack_bf16(ov.x, ov.y);
-        pk.y = pack_bf16(ov.z, ov.w);
-        reinterpret_cast<uint2*>(p.hb + static_cast<long long>(row) * kMegaD)[i * 32 + lane] = pk;
-      }
-    }
-    if (lane == 0) {
-      // loop state: the row that draws the last ticket advances it (same protocol as greedy_select_kernel)
-      if (nxt != p.eos) atomicAdd(&st->not_eos, 1);
-      __threadfence();
-      const unsigned int tr = atomicAdd(&st->ticket, 1u);
-      if (tr == static_cast<unsigned int>(R) - 1) {
-        __threadfence();
-        const int not_eos = atomicAdd(&st->not_eos, 0);
-        st->ticket = 0;
-        st->not_eos = 0;
-        st->cur_len = cur_len + 1;
-        st->final_len = cur_len + 1;
-        st->pos = pos + 1;
-        st->step = step + 1;
-        if (not_eos == 0) {
-          st->finished = 1;
-          if (step == 0 && p.row_prefix == nullptr) st->empty_caption = 1;
-        }
-        if (cur_len + 1 >= p.max_steps) st->finished = 1;
-        __threadfence();
-      }
-    }
+    for (int o2 = 16; o2 > 0; o2 >>= 1)
+      merge_stats(gm, gs, ga, __shfl_xor_sync(0xffffffffu, gm, o2), __shfl_xor_sync(0xffffffffu, gs, o2),
+                  __shfl_xor_sync(0xffffffffu, ga, o2));
+    const RowStep rs = row_step(p.sel, row, step, cur_len, p.sel.next_token[row]);
+    const RowChoice c = resolve_row(p.sel, row, cur_len, rs, ga, -logf(gs));
+    embed_ln_row<kMegaD>(c.nxt, pos + 1, p.words, p.positions, p.lnemb_g, p.lnemb_b, p.sel.V, p.x, p.hb, 0, row, lane);
+    if (lane == 0) commit_row(p.sel, row, step, cur_len, c, nullptr);
   }
 }
 

@@ -1093,7 +1093,8 @@ extern "C" int gitb200_finalize_weights(gitb200_engine* h, void* stream) {
       TRY(pack(l.m_wqkv, l.wqkv, h->D, 3 * h->D, 0, 3 * h->D / 8, 1, 0));
       TRY(pack(l.m_wo, l.wo, h->D, h->D, 0, h->D / 8, 1, 0));
       TRY(pack(l.m_w1, l.w1, h->D, h->F, 0, h->F / 8, 1, 0));
-      for (int sl = 0; sl < 4; ++sl) TRY(pack(l.m_w2, l.w2, h->F, h->D, sl * kMegaD, h->D / 8, 4, sl));
+      for (int sl = 0; sl < kMegaFc2Slices; ++sl)   // k slice sl of feature tile f goes to tile mega_w2_tile(f, sl)
+        TRY(pack(l.m_w2, l.w2, h->F, h->D, sl * kMegaD, h->D / 8, kMegaFc2Slices, sl));
     }
     TRY(pack(h->m_lm, h->words_bf16, h->D, h->V, 0, (h->V + 7) / 8, 1, 0));
     h->mega_ready = true;

@@ -17,8 +17,29 @@ struct StepState {
   int empty_caption;  // greedy step-0 special case (reference layers/decoder.py:279-291)
   unsigned int ticket;
   int not_eos;        // rows whose newest token is not EOS (per step, reset by the last block)
-  int error;          // decode_mega_kernel: a bounded wait gave up (1 grid barrier, 2 ring consumer, 3 ring producer)
+  int error;          // decode_mega_kernel: the MegaWaitError of the first bounded wait that gave up (0: none)
 };
+
+// Why a bounded wait of decode_mega_kernel gave up: a protocol bug ends in one of these codes, not in a hung device.
+enum MegaWaitError : int {
+  kWaitGridBarrier = 1,   // a compute thread at a grid barrier between phases
+  kWaitRingFull = 2,      // a compute warp waiting for a ring chunk to land
+  kWaitRingEmpty = 3,     // the producer waiting for the compute warps to free a ring slot
+  kWaitTextKv = 4,        // the producer waiting for the layer's QKV phase before it fetches the text K/V
+  kWaitRingArmed = 5,     // a compute warp waiting for the producer to arm an attention chunk
+  kWaitTimelineProbe = 99 // timeline build only: the probe that makes a mark wait for the A operand's loads
+};
+inline const char* mega_wait_error_name(int code) {
+  switch (code) {
+    case kWaitGridBarrier: return "grid barrier";
+    case kWaitRingFull: return "ring consumer: chunk never landed";
+    case kWaitRingEmpty: return "ring producer: slot never freed";
+    case kWaitTextKv: return "ring producer: text K/V never written";
+    case kWaitRingArmed: return "ring consumer: attention chunk never armed";
+    case kWaitTimelineProbe: return "timeline probe";
+    default: return "unknown code";
+  }
+}
 
 struct LnParams {
   const float* x;        // [rows, D] fp32 (ldx == D)
@@ -385,28 +406,15 @@ cls_pos_lnpre_kernel(float* __restrict__ x, const float* __restrict__ cls, const
   }
 }
 
-// e = LN(words[tok] + positions[pos], eps 1e-8) (reference layers/decoder.py:65-78); one warp per row.
-// tokens come from `tokens` (int64 [rows], stride tok_stride) ; position = pos_base + (state ? state->pos : 0).
+// One embedded row: e = LN(words[tok] + positions[pos], eps 1e-8) (reference layers/decoder.py:65-78), the token clamped
+// to the vocabulary, stored to output row `row` by ln_store.  One warp.
 template <int D>
-__global__ void __launch_bounds__(256)
-embed_ln_kernel(const long long* __restrict__ tokens, long long tok_stride, const float* __restrict__ words,
-                const float* __restrict__ positions, const float* __restrict__ gamma, const float* __restrict__ beta,
-                float* __restrict__ out_f32, __nv_bfloat16* __restrict__ out_bf16, int rows, int pos_base,
-                const StepState* __restrict__ state, int vocab, int split3, const ChainSync chain) {
+__device__ __forceinline__ void embed_ln_row(long long tok, int pos, const float* __restrict__ words,
+                                             const float* __restrict__ positions, const float* __restrict__ gamma,
+                                             const float* __restrict__ beta, int vocab, float* __restrict__ out_f32,
+                                             __nv_bfloat16* __restrict__ out_bf16, int split3, long long row, int lane) {
   constexpr int NV = D / 128;
-  griddep_launch();
-  griddep_wait();   // chain head: ordered after the previous step by a full dependency
-  tl_mark(4);
-  if (state != nullptr && state->finished) return;
-  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (row >= rows) {
-    chain_signal(chain);
-    return;
-  }
-  const int lane = threadIdx.x & 31;
-  long long tok = tokens[row * tok_stride];
   tok = tok < 0 ? 0 : (tok >= vocab ? vocab - 1 : tok);
-  const int pos = pos_base + (state != nullptr ? state->pos : 0);
   const float4* wp = reinterpret_cast<const float4*>(words + tok * D);
   const float4* pp = reinterpret_cast<const float4*>(positions + static_cast<long long>(pos) * D);
   float4 v[NV];
@@ -422,9 +430,30 @@ embed_ln_kernel(const long long* __restrict__ tokens, long long tok_stride, cons
   for (int i = 0; i < NV; ++i) {
     const float4 g = __ldg(reinterpret_cast<const float4*>(gamma) + i * 32 + lane);
     const float4 b = __ldg(reinterpret_cast<const float4*>(beta) + i * 32 + lane);
-    const float4 o = ln_norm(v[i], mean, rstd, g, b);
-    ln_store<D>(out_f32, out_bf16, split3, row, i * 32 + lane, o);
+    ln_store<D>(out_f32, out_bf16, split3, row, i * 32 + lane, ln_norm(v[i], mean, rstd, g, b));
   }
+}
+
+// The step's input embedding, one warp per row: tokens come from `tokens` (int64 [rows], stride tok_stride); position =
+// pos_base + (state ? state->pos : 0).
+template <int D>
+__global__ void __launch_bounds__(256)
+embed_ln_kernel(const long long* __restrict__ tokens, long long tok_stride, const float* __restrict__ words,
+                const float* __restrict__ positions, const float* __restrict__ gamma, const float* __restrict__ beta,
+                float* __restrict__ out_f32, __nv_bfloat16* __restrict__ out_bf16, int rows, int pos_base,
+                const StepState* __restrict__ state, int vocab, int split3, const ChainSync chain) {
+  griddep_launch();
+  griddep_wait();   // chain head: ordered after the previous step by a full dependency
+  tl_mark(4);
+  if (state != nullptr && state->finished) return;
+  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) {
+    chain_signal(chain);
+    return;
+  }
+  const int pos = pos_base + (state != nullptr ? state->pos : 0);
+  embed_ln_row<D>(tokens[row * tok_stride], pos, words, positions, gamma, beta, vocab, out_f32, out_bf16, split3, row,
+                  threadIdx.x & 31);
   chain_signal(chain);
 }
 
@@ -439,32 +468,12 @@ embed_ln_rows_kernel(const long long* __restrict__ tokens, int T, const float* _
                      const float* __restrict__ positions, const float* __restrict__ gamma, const float* __restrict__ beta,
                      float* __restrict__ out_f32, __nv_bfloat16* __restrict__ out_bf16, int rows, int vocab, int split3,
                      int* __restrict__ targets) {
-  constexpr int NV = D / 128;
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= rows) return;
   const int lane = threadIdx.x & 31;
   const int pos = row % T;
-  long long tok = tokens[row];
-  tok = tok < 0 ? 0 : (tok >= vocab ? vocab - 1 : tok);
   if (lane == 0) targets[row] = pos + 1 < T ? static_cast<int>(tokens[row + 1]) : -1;
-  const float4* wp = reinterpret_cast<const float4*>(words + tok * D);
-  const float4* pp = reinterpret_cast<const float4*>(positions + static_cast<long long>(pos) * D);
-  float4 v[NV];
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const float4 a = __ldg(wp + i * 32 + lane);
-    const float4 b = __ldg(pp + i * 32 + lane);
-    v[i] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
-  }
-  float mean, rstd;
-  ln_row_stats<D>(v, 1e-8f, mean, rstd);
-#pragma unroll
-  for (int i = 0; i < NV; ++i) {
-    const float4 g = __ldg(reinterpret_cast<const float4*>(gamma) + i * 32 + lane);
-    const float4 b = __ldg(reinterpret_cast<const float4*>(beta) + i * 32 + lane);
-    const float4 o = ln_norm(v[i], mean, rstd, g, b);
-    ln_store<D>(out_f32, out_bf16, split3, row, i * 32 + lane, o);
-  }
+  embed_ln_row<D>(tokens[row], pos, words, positions, gamma, beta, vocab, out_f32, out_bf16, split3, row, lane);
 }
 
 // One warp per text row: folds the row's n_parts LM-head partials (gemm.cuh EPI_LSE) into lse, the target's log-probability
@@ -584,6 +593,84 @@ struct SelectParams {
   ChainSync chain;          // last kernel of the chain: waits, then re-zeroes all counters when the step is over
 };
 
+// Pairwise merge of two online-softmax partials (max, sum exp(x - max), arg max); an empty partial has max -inf, and the
+// lowest index wins exact ties of the maximum.
+__device__ __forceinline__ void merge_stats(float& m, float& s, int& a, float m_o, float s_o, int a_o) {
+  const float mn = fmaxf(m, m_o);
+  const float sa = (m == -INFINITY) ? 0.f : __expf(m - mn);
+  const float sb = (m_o == -INFINITY) ? 0.f : __expf(m_o - mn);
+  s = s * sa + s_o * sb;
+  if (m_o > m || (m_o == m && a_o < a)) a = a_o;
+  m = mn;
+}
+
+// Where row `row` of the launch stands at this step.  in_prefix: it is still fed its prefix.  first: its first real
+// decision (no no-repeat mask).  done: it ended, its input token is EOS (reference :347-351: one-hot EOS distribution).
+struct RowStep {
+  bool in_prefix, first, done;
+};
+__device__ __forceinline__ RowStep row_step(const SelectParams& p, int row, int step, int cur_len, long long last) {
+  const int own_prefix = (p.row_prefix != nullptr) ? p.row_prefix_lens[p.row0 + row] : 0;
+  RowStep r;
+  r.in_prefix = (p.row_prefix != nullptr) && cur_len < own_prefix;
+  r.first = (p.row_prefix != nullptr) ? (cur_len == own_prefix) : (step == 0);
+  r.done = !r.first && !r.in_prefix && last == p.eos;
+  return r;
+}
+
+// The row's token and log-prob at this step, and the token it feeds next (teacher forcing: forced[row, cur_len]).
+struct RowChoice {
+  long long tok, nxt;
+  float lp;
+};
+// Inside the prefix: the next prefix token, nothing to score (log-prob 0).  Done: EOS, log_softmax of the one-hot EOS
+// distribution is exactly 0.  Otherwise the model's choice.
+__device__ __forceinline__ RowChoice resolve_row(const SelectParams& p, int row, int cur_len, const RowStep& rs,
+                                                 long long choice, float choice_lp) {
+  RowChoice c{choice, 0, choice_lp};
+  if (rs.in_prefix) {
+    c.tok = p.row_prefix[static_cast<long long>(p.row0 + row) * p.row_prefix_stride + cur_len];
+    c.lp = 0.f;
+  } else if (rs.done) {
+    c.tok = p.eos;
+    c.lp = 0.f;
+  }
+  c.nxt = (p.forced != nullptr) ? p.forced[static_cast<long long>(row) * p.max_steps + cur_len] : c.tok;
+  return c;
+}
+
+// Commits one row's choice; the row that draws the step's last ticket advances the loop state (the reference stops once
+// every token it feeds next is EOS) and re-zeroes the chain counters (null: none).
+__device__ __forceinline__ void commit_row(const SelectParams& p, int row, int step, int cur_len, const RowChoice& c,
+                                           unsigned int* chain_counters) {
+  StepState* st = p.state;
+  p.tokens_out[static_cast<long long>(row) * p.max_steps + cur_len] = c.tok;
+  p.logprob_sum[row] += c.lp;
+  p.next_token[row] = c.nxt;
+  if (c.nxt != p.eos) atomicAdd(&st->not_eos, 1);
+  __threadfence();
+  const unsigned int tr = atomicAdd(&st->ticket, 1u);
+  if (tr == static_cast<unsigned int>(p.rows) - 1) {
+    __threadfence();
+    const int not_eos = atomicAdd(&st->not_eos, 0);
+    st->ticket = 0;
+    st->not_eos = 0;
+    st->cur_len = cur_len + 1;
+    st->final_len = cur_len + 1;
+    st->pos = st->pos + 1;
+    st->step = step + 1;
+    if (not_eos == 0) {
+      st->finished = 1;
+      if (step == 0 && p.row_prefix == nullptr) st->empty_caption = 1;
+    }
+    if (cur_len + 1 >= p.max_steps) st->finished = 1;
+    // every CTA of every kernel of this step has passed its wait: recycle the chain counters
+    if (chain_counters != nullptr)
+      for (int k = 0; k < 64; ++k) chain_counters[k] = 0;
+    __threadfence();
+  }
+}
+
 // grid (n_split, rows): each CTA folds one vocabulary slice of one row into (max, argmax, sum exp) with a
 // single online pass; the last CTA of a row combines the slices and does the reference's bookkeeping.
 __global__ void __launch_bounds__(256) greedy_select_kernel(const SelectParams p) {
@@ -607,9 +694,7 @@ __global__ void __launch_bounds__(256) greedy_select_kernel(const SelectParams p
   // The input token of this step (== our previous choice unless teacher forcing is on): the reference's
   // masks are functions of the *input* sequence (predictions_so_far[:, -1]).
   const long long last = p.next_token[row];
-  const int own_prefix = (p.row_prefix != nullptr) ? p.row_prefix_lens[p.row0 + row] : 0;
-  const bool in_prefix = (p.row_prefix != nullptr) && cur_len < own_prefix;
-  const bool first = (p.row_prefix != nullptr) ? (cur_len == own_prefix) : (step == 0);   // the row's first real decision
+  const RowStep rs = row_step(p, row, step, cur_len, last);
   const int chunk = (p.V + p.n_split - 1) / p.n_split;
   const int lo = split * chunk;
   const int hi = min(p.V, lo + chunk);
@@ -625,7 +710,7 @@ __global__ void __launch_bounds__(256) greedy_select_kernel(const SelectParams p
     for (int u = 0; u < 16; ++u) {
       const int i = i0 + u * 256;
       v[u] = (i < hi) ? __ldcg(z + i) : -INFINITY;
-      if (!first && i == static_cast<int>(last)) v[u] = -10000.0f;   // no-repeat (reference :330)
+      if (!rs.first && i == static_cast<int>(last)) v[u] = -10000.0f;   // no-repeat (reference :330)
     }
 #pragma unroll
     for (int u = 0; u < 16; ++u) {
@@ -643,28 +728,13 @@ __global__ void __launch_bounds__(256) greedy_select_kernel(const SelectParams p
   __shared__ float s_m[8], s_s[8];
   __shared__ int s_a[8];
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float m_o = __shfl_xor_sync(0xffffffffu, m, o);
-    const float s_o = __shfl_xor_sync(0xffffffffu, ssum, o);
-    const int a_o = __shfl_xor_sync(0xffffffffu, arg, o);
-    const float mn = fmaxf(m, m_o);
-    const float sa = (m == -INFINITY) ? 0.f : __expf(m - mn);
-    const float sb = (m_o == -INFINITY) ? 0.f : __expf(m_o - mn);
-    ssum = ssum * sa + s_o * sb;
-    if (m_o > m || (m_o == m && a_o < arg)) arg = a_o;
-    m = mn;
-  }
+  for (int o = 16; o > 0; o >>= 1)
+    merge_stats(m, ssum, arg, __shfl_xor_sync(0xffffffffu, m, o), __shfl_xor_sync(0xffffffffu, ssum, o),
+                __shfl_xor_sync(0xffffffffu, arg, o));
   if ((tid & 31) == 0) { s_m[tid >> 5] = m; s_s[tid >> 5] = ssum; s_a[tid >> 5] = arg; }
   __syncthreads();
   if (tid == 0) {
-    for (int w = 1; w < 8; ++w) {
-      const float mn = fmaxf(m, s_m[w]);
-      const float sa = (m == -INFINITY) ? 0.f : __expf(m - mn);
-      const float sb = (s_m[w] == -INFINITY) ? 0.f : __expf(s_m[w] - mn);
-      ssum = ssum * sa + s_s[w] * sb;
-      if (s_m[w] > m || (s_m[w] == m && s_a[w] < arg)) arg = s_a[w];
-      m = mn;
-    }
+    for (int w = 1; w < 8; ++w) merge_stats(m, ssum, arg, s_m[w], s_s[w], s_a[w]);
     p.part_max[row * p.n_split + split] = m;
     p.part_sum[row * p.n_split + split] = ssum;
     p.part_arg[row * p.n_split + split] = arg;
@@ -673,61 +743,14 @@ __global__ void __launch_bounds__(256) greedy_select_kernel(const SelectParams p
     if (t == static_cast<unsigned int>(p.n_split) - 1) {
       __threadfence();
       p.row_ticket[row] = 0;
-      // combine the slices (slice order = index order, so ">" keeps the lowest index on ties)
+      // combine the slices in slice order (= index order); a row without a finite logit keeps arg 0
       float gm = -INFINITY, gs = 0.f;
       int ga = 0;
-      for (int k = 0; k < p.n_split; ++k) {
-        const float pm = __ldcg(&p.part_max[row * p.n_split + k]);
-        const float ps = __ldcg(&p.part_sum[row * p.n_split + k]);
-        const int pa = __ldcg(&p.part_arg[row * p.n_split + k]);
-        const float mn = fmaxf(gm, pm);
-        const float sa = (gm == -INFINITY) ? 0.f : __expf(gm - mn);
-        const float sb = (pm == -INFINITY) ? 0.f : __expf(pm - mn);
-        gs = gs * sa + ps * sb;
-        if (pm > gm) ga = pa;
-        gm = mn;
-      }
-      const bool row_done = (!first) && (!in_prefix) && (last == p.eos);
-      long long tok;
-      float lp;
-      if (in_prefix) {   // still feeding this row's prefix: the next prefix token, nothing to score
-        tok = p.row_prefix[static_cast<long long>(p.row0 + row) * p.row_prefix_stride + cur_len];
-        lp = 0.f;
-      } else if (row_done) {  // one-hot EOS distribution (reference :347-351): log_softmax gives exactly 0 at EOS
-        tok = p.eos;
-        lp = 0.f;
-      } else {
-        tok = ga;
-        lp = -logf(gs);  // z[arg] - max - log(sum exp(z - max)) with z[arg] == max
-      }
-      p.tokens_out[static_cast<long long>(row) * p.max_steps + cur_len] = tok;
-      p.logprob_sum[row] += lp;
-      long long nxt = tok;
-      if (p.forced != nullptr) nxt = p.forced[static_cast<long long>(row) * p.max_steps + cur_len];
-      p.next_token[row] = nxt;
-      // reference checks `(last_predictions == eos).all()` on the sequence it feeds next
-      if (nxt != p.eos) atomicAdd(&st->not_eos, 1);
-      __threadfence();
-      const unsigned int tr = atomicAdd(&st->ticket, 1u);
-      if (tr == static_cast<unsigned int>(p.rows) - 1) {  // last row of this step: advance the loop state
-        __threadfence();
-        const int not_eos = atomicAdd(&st->not_eos, 0);
-        st->ticket = 0;
-        st->not_eos = 0;
-        st->cur_len = cur_len + 1;
-        st->final_len = cur_len + 1;
-        st->pos = st->pos + 1;
-        st->step = step + 1;
-        if (not_eos == 0) {
-          st->finished = 1;
-          if (step == 0 && p.row_prefix == nullptr) st->empty_caption = 1;
-        }
-        if (cur_len + 1 >= p.max_steps) st->finished = 1;
-        // every CTA of every kernel of this step has passed its wait: recycle the chain counters
-        if (p.chain.counters != nullptr)
-          for (int k = 0; k < 64; ++k) p.chain.counters[k] = 0;
-        __threadfence();
-      }
+      for (int k = 0; k < p.n_split; ++k)
+        merge_stats(gm, gs, ga, __ldcg(&p.part_max[row * p.n_split + k]), __ldcg(&p.part_sum[row * p.n_split + k]),
+                    __ldcg(&p.part_arg[row * p.n_split + k]));
+      // z[arg] - max - log(sum exp(z - max)) with z[arg] == max
+      commit_row(p, row, step, cur_len, resolve_row(p, row, cur_len, rs, ga, -logf(gs)), p.chain.counters);
     }
   }
 }
