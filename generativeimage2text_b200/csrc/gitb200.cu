@@ -20,6 +20,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -52,6 +53,7 @@ typedef __nv_bfloat16 bf16;
 static thread_local std::string g_create_error;
 
 struct DevBuf {
+  static inline std::atomic<unsigned long long> moves{0};   // bumped whenever a buffer's address changes (step_graph)
   void* p = nullptr;
   size_t cap = 0;
   bool owned = true;   // false: borrowed from another engine (gitb200_share_weights)
@@ -61,11 +63,13 @@ struct DevBuf {
     if (p) cudaFree(p);
     p = nullptr;
     cap = 0;
+    ++moves;
     cudaError_t e = cudaMalloc(&p, bytes);
     if (e == cudaSuccess) cap = bytes;
     return e;
   }
   void release() {
+    if (p) ++moves;
     if (p && owned) cudaFree(p);
     p = nullptr;
     cap = 0;
@@ -73,6 +77,7 @@ struct DevBuf {
   }
   void borrow(const DevBuf& o) {
     release();
+    ++moves;
     p = o.p;
     cap = o.cap;
     owned = false;
@@ -138,9 +143,7 @@ struct gitb200_engine {
   // input size of the next encode (gitb200_set_input_size; default image_size x image_size): patch grid gh x gw,
   // Lc = gh * gw + 1 tokens per image; differs from (g, g, L) for MinMaxResizeForTest inputs (reference inference.py:29-64)
   int in_h = 0, in_w = 0, gh = 0, gw = 0, Lc = 0;
-  // ragged batches: (height, width) of every image of the NEXT encode / generate (gitb200_set_image_sizes; consumed by it),
-  // and the per-image tables of the last encode (cur_ragged: its images had their own sizes; RaggedImg [B], L_b [B])
-  std::vector<int> rg_next_hw;
+  // per-image tables of the last encode when its images had their own sizes (cur_ragged): RaggedImg [B], L_b [B]
   bool cur_ragged = false;
   std::vector<int> cur_lens;
   DevBuf rg_tab, rg_lens;
@@ -177,10 +180,10 @@ struct gitb200_engine {
   std::map<TmapKey, CUtensorMap> tmaps;
 
   // decode-step graph cache
-  // (a call's graph is keyed by its row count, cache geometry and buffer addresses; several shapes alternate when batches
-  //  are coalesced into launches of different sizes, so a handful of instantiated graphs are kept)
+  // (keyed by everything the captured launches bake in, see step_graph; several shapes alternate when batches are
+  //  coalesced into launches of different sizes, so a handful of instantiated graphs are kept)
   struct StepGraph { cudaGraphExec_t exec = nullptr; int64_t launches = 0; unsigned long long last_use = 0; };
-  std::map<std::vector<long long>, StepGraph> step_graphs;
+  std::map<std::string, StepGraph> step_graphs;
   unsigned long long step_graph_clock = 0;
   int last_gemm_grid = 0;
   cudaStream_t own_stream = nullptr;
@@ -195,19 +198,28 @@ struct gitb200_engine {
   cudaEvent_t dec_ev[2] = {nullptr, nullptr};     // around the decode loop of the last generate (gitb200_last_decode_ms)
   int dec_steps = 0;                               // step launches between them
   bool dec_mega = false;                           // ... each of which was one decode_mega_kernel launch
-  // per-row prefixes of the NEXT generate call (gitb200_set_row_prefixes; consumed by that call)
-  const int64_t* rp_tok = nullptr;
-  const int32_t* rp_lens = nullptr;
-  int rp_rows = 0, rp_stride = 0;
-  // vocabulary trie (gitb200_set_trie; sticky) and the uniforms of the next sampled generate (gitb200_set_sampling)
+  // vocabulary trie (gitb200_set_trie; sticky)
   DevBuf trie_begin, trie_token, trie_child, trie_cursor;
   int trie_nodes = 0;
-  const float* sample_u = nullptr;
-  int sample_steps = 0, sample_rows = 0;
-  float sample_temperature = 1.0f;
-  bool constrained = false;            // this call's greedy selection runs constrained_select_kernel
-  int64_t* pend_tok_host = nullptr;  // host-buffer variant: results land here
+  // inputs of the next call only, taken by it at entry (take_next_call)
+  struct NextCall {
+    std::vector<int> image_hw;           // (height, width) of every image (gitb200_set_image_sizes)
+    const long long* prefix_tok = nullptr;  // per-row prefixes (gitb200_set_row_prefixes)
+    const int32_t* prefix_lens = nullptr;
+    int prefix_rows = 0, prefix_stride = 0;
+    const float* uniforms = nullptr;      // sampling (gitb200_set_sampling)
+    int sample_steps = 0, sample_rows = 0;
+    float temperature = 1.0f;
+  } next;
 };
+
+// The inputs set for the next call that the calling one takes (include/gitb200.h, gitb200_set_image_sizes).
+static gitb200_engine::NextCall take_next_call(gitb200_engine* h, bool generate) {
+  gitb200_engine::NextCall c;
+  if (generate) std::swap(c, h->next);
+  else c.image_hw.swap(h->next.image_hw);
+  return c;
+}
 
 static void drop_step_graphs(gitb200_engine* h) {
   for (auto& kv : h->step_graphs) if (kv.second.exec) cudaGraphExecDestroy(kv.second.exec);
@@ -813,7 +825,7 @@ extern "C" int gitb200_set_image_sizes(gitb200_engine* h, const int32_t* hw_host
     const long long tokens = static_cast<long long>(ih / p) * (iw / p) + 1;
     if (tokens > 16384) return fail(h, "set_image_sizes: image %d (%dx%d) gives %lld tokens (limit 16384)", b, ih, iw, tokens);
   }
-  h->rg_next_hw.swap(hw);
+  h->next.image_hw.swap(hw);
   return 0;
 }
 

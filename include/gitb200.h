@@ -104,8 +104,10 @@ int gitb200_set_input_size(gitb200_engine* h, int height, int width);
  * images (images_dev or the host buffer) hold the n images back to back, fp32 [3, H_b, W_b] each; its batch must equal n
  * and frames must be 0 or 1.  Image b has L_b = (H_b / patch) * (W_b / patch) + 1 tokens in a slot of L_max = max L_b
  * rows: row b of the results is what a batch-1 call with that image alone returns.  The greedy decode steps of such a
- * call run on the kernel chain (use_mega does not apply).  Applies to the next call only, like gitb200_set_row_prefixes;
- * gitb200_set_input_size is left as it was. */
+ * call run on the kernel chain (use_mega does not apply).  gitb200_set_input_size is left as it was.
+ * Inputs of the next call only (this one, gitb200_set_row_prefixes, gitb200_set_sampling): the next call that can use
+ * them takes them at entry, right after its in-flight check -- gitb200_encode and gitb200_score take the image sizes, a
+ * gitb200_generate* call takes all three -- and they are gone from the engine whether that call succeeds or fails. */
 int gitb200_set_image_sizes(gitb200_engine* h, const int32_t* hw_host, int n);
 
 /* Replaces: visual_projection + the image rows of BertEncoderAsDecoder, computed once (KV cache)
@@ -173,11 +175,11 @@ int gitb200_score(gitb200_engine* h, const float* images_dev, int batch, int fra
  * was the single decode_mega_kernel launch.  Waits for that loop to finish.  No reference counterpart. */
 int gitb200_last_decode_ms(gitb200_engine* h, float* ms_out, int32_t* steps_out, int32_t* one_kernel_out);
 
-/* Per-row prefixes for the NEXT generate call (question batches; the reference allows one prefix and batch 1 only,
- * layers/decoder.py:985-1006): prefix_dev int64 [rows, stride], lens_dev int32 [rows] (1 <= len <= stride, len < max_steps;
- * tokens past a row's length are ignored).  rows must equal that call's batch; pass prefix_len = 0 to it.  Every row is
- * generated exactly as a batch-1 call with its own prefix would be; tokens_out rows hold prefix + generated tokens.  The
- * buffers must stay valid until the call has finished. */
+/* Per-row prefixes for the NEXT generate call, which takes them as gitb200_set_image_sizes describes (question batches;
+ * the reference allows one prefix and batch 1 only, layers/decoder.py:985-1006): prefix_dev int64 [rows, stride],
+ * lens_dev int32 [rows] (1 <= len <= stride, len < max_steps; tokens past a row's length are ignored).  rows must equal
+ * that call's batch; pass prefix_len = 0 to it.  Every row is generated exactly as a batch-1 call with its own prefix
+ * would be; tokens_out rows hold prefix + generated tokens.  The buffers must stay valid until the call has finished. */
 int gitb200_set_row_prefixes(gitb200_engine* h, const int64_t* prefix_dev, int rows, int stride, const int32_t* lens_dev);
 
 /* Replaces: TrieAutoRegressiveBeamSearch.search + TokenTrie                            trie_decoder.py:27-258
@@ -191,11 +193,11 @@ int gitb200_set_trie(gitb200_engine* h, const int32_t* child_begin_host, const i
                      const int32_t* child_node_host, int n_nodes, int n_edges);
 
 /* Replaces: the do_sample branches of AutoRegressiveBeamSearch.search            layers/decoder.py:260-272, 364-375
- * for the NEXT greedy generate call: row r draws its token at caption length t from softmax(logits / temperature) by an
- * inverse-CDF lookup in index order with uniforms_dev[t * rows + r] (fp32 [steps >= max_steps, rows == batch], device;
- * torch.multinomial's random stream cannot be reproduced, the distribution is the same).  Log-probs as the reference
- * computes them: tempered log-softmax at a row's first decision, un-tempered afterwards.  The buffer must stay valid
- * until the call has finished. */
+ * for the NEXT generate call, which must be greedy and takes them as gitb200_set_image_sizes describes: row r draws its
+ * token at caption length t from softmax(logits / temperature) by an inverse-CDF lookup in index order with
+ * uniforms_dev[t * rows + r] (fp32 [steps >= max_steps, rows == batch], device; torch.multinomial's random stream cannot
+ * be reproduced, the distribution is the same).  Log-probs as the reference computes them: tempered log-softmax at a
+ * row's first decision, un-tempered afterwards.  The buffer must stay valid until the call has finished. */
 int gitb200_set_sampling(gitb200_engine* h, const float* uniforms_dev, int steps, int rows, float temperature);
 
 /* Number of kernels the engine launched since creation (bench.py's gpu_launches). */
