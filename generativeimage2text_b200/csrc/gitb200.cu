@@ -111,6 +111,19 @@ struct TmapKey {
   }
 };
 
+// The images of one call as the encoder reads them (image_batch), built at the call's entry from its batch and frames and
+// either the sizes set for it (gitb200_set_image_sizes) or the sticky input size (gitb200_set_input_size).
+struct ImageBatch {
+  std::vector<RaggedImg> imgs;   // every encoded image, NI = B * frames of them in the encoder's order f * B + b
+  int B = 0, frames = 1;         // frames after the temporal-embedding truncation of list inputs
+  int L_max = 0;                 // slot length: tokens of the largest image
+  std::vector<int> lens;         // a ragged batch: L of each image (rg_lens), else empty
+  int pos_rows = 0;              // rows of the call's positional table in pos_interp (0: the stored table serves)
+  size_t bytes = 0;              // pixel bytes the call passes (every frame, before the truncation)
+  bool list_input = false;       // frames >= 1 were passed: temporal embeddings apply
+  bool ragged = false;           // the sizes were given per image
+};
+
 // Geometry of decode_attn_kernel (dec_attn_geometry).
 struct DecAttnGeom {
   int chunk_rows, box_rows;   // DecAttnParams::chunk_rows / box_rows
@@ -140,13 +153,15 @@ struct gitb200_engine {
 
   // derived geometry
   int g = 0, L = 0, Kpatch = 0, Kp = 0, d = 0, D = 0, F = 0, V = 0;
-  // input size of the next encode (gitb200_set_input_size; default image_size x image_size): patch grid gh x gw,
-  // Lc = gh * gw + 1 tokens per image; differs from (g, g, L) for MinMaxResizeForTest inputs (reference inference.py:29-64)
-  int in_h = 0, in_w = 0, gh = 0, gw = 0, Lc = 0;
-  // per-image tables of the last encode when its images had their own sizes (cur_ragged): RaggedImg [B], L_b [B]
-  bool cur_ragged = false;
-  std::vector<int> cur_lens;
+  // input size of the next encodes (gitb200_set_input_size; default image_size x image_size); differs from the model's
+  // for MinMaxResizeForTest inputs (reference inference.py:29-64)
+  int in_h = 0, in_w = 0;
+  // the images of the last encode (cur_img.ragged: their sizes were given per image) and, on the device, its RaggedImg
+  // table and, for a ragged batch, each image's valid key count L_b; what the last upload wrote to each, so that a call
+  // with the same images copies nothing
+  ImageBatch cur_img;
   DevBuf rg_tab, rg_lens;
+  std::string rg_tab_up, rg_lens_up;
 
   // weights
   DevBuf w_patch, cls, pos_emb, lnpre_g, lnpre_b, lnpost_g, lnpost_b;
@@ -159,7 +174,6 @@ struct gitb200_engine {
 
   // workspaces
   DevBuf x, h, qkv, ctx, u, feats, feats_f32, pos_interp;   // encoder
-  int pos_rows = 0;                                         // rows of pos_interp the last encode re-sampled (0: none)
   DevBuf pt, pxd, phd, pq, pctx, pu;                        // decoder-layer pass (image rows, caption rows)
   DevBuf img_kv, txt_kv, src_row[2];                        // caches
   size_t txt_kv_eb = 0;                                     // element size (kvb()) the text cache was last zeroed for
@@ -798,18 +812,26 @@ extern "C" int gitb200_set_option(gitb200_engine* h, const char* name, int64_t v
   return fail(h, "unknown option %s", name);
 }
 
+// The size checks of both size setters: 0, or fails with "<what>: <image><size> ..." (image: "" or "image b ").
+static int check_image_size(gitb200_engine* h, const char* what, int b, int height, int width) {
+  const int p = h->cfg.patch;
+  const long long tokens = static_cast<long long>(height / p) * (width / p) + 1;
+  if (b < 0) {
+    if (height < p || width < p) return fail(h, "%s: %dx%d is smaller than one %dx%d patch", what, height, width, p, p);
+    if (tokens > 16384) return fail(h, "%s: %dx%d gives %lld tokens per image (limit 16384)", what, height, width, tokens);
+    return 0;
+  }
+  if (height < p || width < p) return fail(h, "%s: image %d is %dx%d, smaller than one %dx%d patch", what, b, height, width, p, p);
+  if (tokens > 16384) return fail(h, "%s: image %d (%dx%d) gives %lld tokens (limit 16384)", what, b, height, width, tokens);
+  return 0;
+}
+
 extern "C" int gitb200_set_input_size(gitb200_engine* h, int height, int width) {
   if (!h) return 1;
   if (h->pending) return fail(h, "set_input_size: a generate call is in flight");
-  const int p = h->cfg.patch;
-  if (height < p || width < p) return fail(h, "set_input_size: %dx%d is smaller than one %dx%d patch", height, width, p, p);
-  const long long tokens = static_cast<long long>(height / p) * (width / p) + 1;
-  if (tokens > 16384) return fail(h, "set_input_size: %dx%d gives %lld tokens per image (limit 16384)", height, width, tokens);
+  TRY(check_image_size(h, "set_input_size", -1, height, width));
   h->in_h = height;
   h->in_w = width;
-  h->gh = height / p;      // nn.Conv2d(kernel = stride = patch, no padding) drops a trailing partial patch
-  h->gw = width / p;
-  h->Lc = h->gh * h->gw + 1;
   return 0;
 }
 
@@ -817,15 +839,8 @@ extern "C" int gitb200_set_image_sizes(gitb200_engine* h, const int32_t* hw_host
   if (!h) return 1;
   if (h->pending) return fail(h, "set_image_sizes: a generate call is in flight");
   if (!hw_host || n < 1) return fail(h, "set_image_sizes: bad argument");
-  const int p = h->cfg.patch;
-  std::vector<int> hw(hw_host, hw_host + 2 * n);
-  for (int b = 0; b < n; ++b) {
-    const int ih = hw[2 * b], iw = hw[2 * b + 1];
-    if (ih < p || iw < p) return fail(h, "set_image_sizes: image %d is %dx%d, smaller than one %dx%d patch", b, ih, iw, p, p);
-    const long long tokens = static_cast<long long>(ih / p) * (iw / p) + 1;
-    if (tokens > 16384) return fail(h, "set_image_sizes: image %d (%dx%d) gives %lld tokens (limit 16384)", b, ih, iw, tokens);
-  }
-  h->next.image_hw.swap(hw);
+  for (int b = 0; b < n; ++b) TRY(check_image_size(h, "set_image_sizes", b, hw_host[2 * b], hw_host[2 * b + 1]));
+  h->next.image_hw.assign(hw_host, hw_host + 2 * n);
   return 0;
 }
 
@@ -852,8 +867,6 @@ extern "C" int gitb200_create(const gitb200_config* cfg, int device, gitb200_eng
   h->g = cfg->image_size / cfg->patch;
   h->L = h->g * h->g + 1;
   h->in_h = h->in_w = cfg->image_size;
-  h->gh = h->gw = h->g;
-  h->Lc = h->L;
   h->Kpatch = 3 * cfg->patch * cfg->patch;
   h->Kp = (h->Kpatch + 63) / 64 * 64;
   h->d = cfg->enc_width;
@@ -1120,78 +1133,104 @@ extern "C" int gitb200_finalize_weights(gitb200_engine* h, void* stream) {
 // ------------------------------------------------------------------------------------------------
 // hot path A: encoder
 // ------------------------------------------------------------------------------------------------
-// Per-image tables of a ragged batch (hw: height, width of every image): RaggedImg [B] and L_b [B] on the device, the
-// positional embedding of every distinct patch grid of the call in h->pos_interp (the stored one copied for the model's
-// own grid, the bicubic re-sampling for any other), and the slot length L_max.
-static int ragged_setup(gitb200_engine* h, const std::vector<int>& hw, int B, int* L_max, cudaStream_t st) {
-  const int p = h->cfg.patch, d = h->d;
-  std::vector<RaggedImg> tab(B);
+// The images of a call (include/gitb200.h gitb200_encode; frames < 1: a bare tensor, no temporal embeddings; hw: empty, or
+// the (height, width) of each of the B images, set for this call by gitb200_set_image_sizes).  Each image gets the row
+// of its grid in the call's positional table (pos_table): every image of the model's own grid reads the stored table,
+// else the table holds one block per distinct grid in order of first appearance.
+static int image_batch(gitb200_engine* h, const char* what, int B, int frames, const std::vector<int>& hw, ImageBatch* out) {
+  ImageBatch& ib = *out;
+  ib.B = B;
+  ib.frames = frames < 1 ? 1 : frames;
+  ib.list_input = frames >= 1;
+  ib.ragged = !hw.empty();
+  if (B < 1) return fail(h, "%s: bad batch/frames", what);
+  if (ib.ragged && (static_cast<int>(hw.size()) != 2 * B || ib.frames != 1))
+    return fail(h, "%s: %d image sizes were set for a batch of %d x %d frames (images of their own sizes take frames 0 or 1)",
+                what, static_cast<int>(hw.size() / 2), B, ib.frames);
+  ib.bytes = 3ULL * h->in_h * h->in_w * B * ib.frames * sizeof(float);
+  if (ib.list_input && h->cfg.num_frames_emb > 0 && ib.frames > h->cfg.num_frames_emb) {
+    // reference zip() truncates to the number of temporal embeddings (layers/decoder.py:848-849)
+    ib.frames = h->cfg.num_frames_emb;
+  }
+  const int p = h->cfg.patch, NI = B * ib.frames;
   std::vector<std::pair<int, int>> grids;     // distinct (gh, gw) in order of first appearance
   std::vector<int> grid_row;                  // their first row in the positional table
-  int rows = 0, Lm = 0;
   long long off = 0;
-  for (int b = 0; b < B; ++b) {
-    RaggedImg& e = tab[b];
-    e.h = hw[2 * b]; e.w = hw[2 * b + 1];
-    e.gh = e.h / p; e.gw = e.w / p;
+  ib.imgs.resize(NI);
+  for (int i = 0; i < NI; ++i) {
+    RaggedImg& e = ib.imgs[i];
+    e.h = ib.ragged ? hw[2 * i] : h->in_h;
+    e.w = ib.ragged ? hw[2 * i + 1] : h->in_w;
+    e.gh = e.h / p;      // nn.Conv2d(kernel = stride = patch, no padding) drops a trailing partial patch
+    e.gw = e.w / p;
     e.L = e.gh * e.gw + 1;
     e.src_off = off;
     off += 3LL * e.h * e.w;
     size_t k = 0;
     while (k < grids.size() && grids[k] != std::make_pair(e.gh, e.gw)) ++k;
-    if (k == grids.size()) { grids.emplace_back(e.gh, e.gw); grid_row.push_back(rows); rows += e.L; }
+    if (k == grids.size()) { grids.emplace_back(e.gh, e.gw); grid_row.push_back(ib.pos_rows); ib.pos_rows += e.L; }
     e.pos_row = grid_row[k];
-    Lm = std::max(Lm, e.L);
+    ib.L_max = std::max(ib.L_max, e.L);
+    if (ib.ragged) ib.lens.push_back(e.L);
   }
-  CK(h->pos_interp.ensure(static_cast<size_t>(rows) * d * 4));
-  for (size_t k = 0; k < grids.size(); ++k) {
-    const int gh = grids[k].first, gw = grids[k].second;
-    float* dst = h->pos_interp.as<float>() + static_cast<size_t>(grid_row[k]) * d;
-    if (gh == h->g && gw == h->g) {
-      CK(cudaMemcpyAsync(dst, h->pos_emb.p, static_cast<size_t>(h->L) * d * 4, cudaMemcpyDeviceToDevice, st));
-      continue;
-    }
-    const long long total = static_cast<long long>(gh * gw + 1) * (d / 4);
-    const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, h->num_sms * 8));
-    pos_embed_bicubic_kernel<<<grid, 256, 0, st>>>(h->pos_emb.as<float>(), dst, h->g, gh, gw, d);
-    CKL(h, "pos_embed_bicubic_kernel");
-  }
-  std::vector<int> lens(B);
-  for (int b = 0; b < B; ++b) lens[b] = tab[b].L;
-  CK(h->rg_tab.ensure(static_cast<size_t>(B) * sizeof(RaggedImg)));
-  CK(h->rg_lens.ensure(static_cast<size_t>(B) * 4));
-  CK(cudaMemcpyAsync(h->rg_tab.p, tab.data(), static_cast<size_t>(B) * sizeof(RaggedImg), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(h->rg_lens.p, lens.data(), static_cast<size_t>(B) * 4, cudaMemcpyHostToDevice, st));
-  h->cur_lens.swap(lens);
-  h->pos_rows = rows;
-  *L_max = Lm;
+  if (ib.ragged) ib.bytes = static_cast<size_t>(off) * sizeof(float);
+  if (grids.size() == 1 && grids[0] == std::make_pair(h->g, h->g)) ib.pos_rows = 0;
   return 0;
 }
 
-// ragged_hw: empty, or (height, width) of each of the B images (gitb200_set_image_sizes; frames must be 1)
-static int encode_impl(gitb200_engine* h, const float* images, int B, int frames, bool list_input, float* feats_out,
-                       cudaStream_t st, const std::vector<int>& ragged_hw = std::vector<int>()) {
-  if (!h->finalized) return fail(h, "weights not finalized");
-  if (B < 1 || frames < 1) return fail(h, "encode: bad batch/frames");
-  const bool rg = !ragged_hw.empty();
-  if (rg && (static_cast<int>(ragged_hw.size()) != 2 * B || frames != 1))
-    return fail(h, "encode: %d image sizes were set for a batch of %d x %d frames (ragged batches take one frame)",
-                static_cast<int>(ragged_hw.size() / 2), B, frames);
-  if (list_input && h->cfg.num_frames_emb > 0 && frames > h->cfg.num_frames_emb) {
-    // reference zip() truncates to the number of temporal embeddings (layers/decoder.py:848-849)
-    frames = h->cfg.num_frames_emb;
+// The positional table of a call's images (image_batch; reference layers/CLIP/model.py:245-251) -> *pos: the stored one,
+// or pos_interp with the stored one copied for the model's own grid and the bicubic re-sampling for any other.  Made on
+// every call: the parameters may have changed.
+static int pos_table(gitb200_engine* h, const ImageBatch& ib, const float** pos, cudaStream_t st) {
+  *pos = h->pos_emb.as<float>();
+  if (ib.pos_rows == 0) return 0;
+  const int d = h->d;
+  CK(h->pos_interp.ensure(static_cast<size_t>(ib.pos_rows) * d * 4));
+  int next = 0;   // the blocks are numbered in order of first appearance: the first image of a grid starts the next one
+  for (const RaggedImg& e : ib.imgs) {
+    if (e.pos_row != next) continue;
+    float* dst = h->pos_interp.as<float>() + static_cast<size_t>(next) * d;
+    next += e.L;
+    if (e.gh == h->g && e.gw == h->g) {
+      CK(cudaMemcpyAsync(dst, h->pos_emb.p, static_cast<size_t>(h->L) * d * 4, cudaMemcpyDeviceToDevice, st));
+      continue;
+    }
+    const long long total = static_cast<long long>(e.L) * (d / 4);
+    const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, h->num_sms * 8));
+    pos_embed_bicubic_kernel<<<grid, 256, 0, st>>>(h->pos_emb.as<float>(), dst, h->g, e.gh, e.gw, d);
+    CKL(h, "pos_embed_bicubic_kernel");
   }
-  h->cur_ragged = false;
-  h->pos_rows = 0;
-  int L = h->Lc;
-  if (rg) TRY(ragged_setup(h, ragged_hw, B, &L, st));
-  const int d = h->d, gh = h->gh, gw = h->gw, Kp = h->Kp, H = h->cfg.enc_heads;
+  *pos = h->pos_interp.as<float>();
+  return 0;
+}
+
+// Copies `bytes` from host memory to buf on `st` unless the last copy through here left exactly these bytes there (last;
+// forgotten when buf is re-allocated or released, which changes its capacity).
+static int upload_changed(gitb200_engine* h, DevBuf& buf, std::string& last, const void* src, size_t bytes, cudaStream_t st) {
+  const size_t cap = buf.cap;
+  CK(buf.ensure(bytes));
+  if (buf.cap != cap) last.clear();
+  if (last.size() == bytes && memcmp(last.data(), src, bytes) == 0) return 0;
+  CK(cudaMemcpyAsync(buf.p, src, bytes, cudaMemcpyHostToDevice, st));
+  last.assign(static_cast<const char*>(src), bytes);
+  return 0;
+}
+
+// Valid image keys of each image on the device when the images of `ib` had their own sizes, else null.
+static const int* img_lens(const gitb200_engine* h, const ImageBatch& ib) { return ib.ragged ? h->rg_lens.as<int>() : nullptr; }
+
+static int encode_impl(gitb200_engine* h, const float* images, const ImageBatch& ib, float* feats_out, cudaStream_t st) {
+  if (!h->finalized) return fail(h, "weights not finalized");
+  h->cur_img.ragged = false;
+  const int B = ib.B, frames = ib.frames, L = ib.L_max;
+  TRY(upload_changed(h, h->rg_tab, h->rg_tab_up, ib.imgs.data(), ib.imgs.size() * sizeof(RaggedImg), st));
+  if (ib.ragged) TRY(upload_changed(h, h->rg_lens, h->rg_lens_up, ib.lens.data(), ib.lens.size() * sizeof(int), st));
+  const int d = h->d, Kp = h->Kp, H = h->cfg.enc_heads;
   const int NI = B * frames;
   const long long Me = static_cast<long long>(NI) * L;
   const int ks = h->ks();                 // parity mode: GEMM operands are [hi | lo | hi] -> 3x the K extent
   const bool par = h->parity;
   const size_t qkv_eb = h->kvb();         // q | k | v: bf16, fp32 in parity mode
-  const int* seq_lens = rg ? h->rg_lens.as<int>() : nullptr;
   CK(h->x.ensure(Me * d * 4));
   CK(h->h.ensure(Me * d * 2 * ks));
   CK(h->qkv.ensure(Me * 3 * d * qkv_eb));
@@ -1202,27 +1241,15 @@ static int encode_impl(gitb200_engine* h, const float* images, int B, int frames
   bf16* hb = h->h.as<bf16>();
   bf16* ctx = h->ctx.as<bf16>();
   bf16* u = h->u.as<bf16>();
-
-  // positional embedding of this input size: the stored one, or its bicubic re-sampling to the gh x gw grid
-  // (reference layers/CLIP/model.py:245-251; recomputed per call: 1 + gh*gw rows, the parameters may have changed)
-  // (ragged batches: one table per distinct grid, made by ragged_setup)
-  const float* pos = rg ? h->pos_interp.as<float>() : h->pos_emb.as<float>();
-  if (!rg && (gh != h->g || gw != h->g)) {
-    CK(h->pos_interp.ensure(static_cast<size_t>(L) * d * 4));
-    const long long total = static_cast<long long>(L) * (d / 4);
-    const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, h->num_sms * 8));
-    pos_embed_bicubic_kernel<<<grid, 256, 0, st>>>(h->pos_emb.as<float>(), h->pos_interp.as<float>(), h->g, gh, gw, d);
-    CKL(h, "pos_embed_bicubic_kernel");
-    pos = h->pos_interp.as<float>();
-    h->pos_rows = L;
-  }
-  // patch embedding: im2col + GEMM, rows land at token index 1 + patch (CLS row is filled by the next kernel)
-  // (ragged batches: every image owns L_max - 1 patch rows, the ones past its own grid are zero)
+  const RaggedImg* tab = h->rg_tab.as<RaggedImg>();
+  const float* pos = nullptr;
+  TRY(pos_table(h, ib, &pos, st));
+  // patch embedding: im2col + GEMM, rows land at token index 1 + patch (CLS row is filled by the next kernel); every image
+  // owns L_max - 1 patch rows, the ones past its own grid are zero
   {
     const long long total = static_cast<long long>(NI) * (L - 1) * (Kp / 8);
     const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, h->num_sms * 16));
-    if (rg) im2col_patch_ragged_kernel<<<grid, 256, 0, st>>>(images, u, h->rg_tab.as<RaggedImg>(), NI, L - 1, h->cfg.patch, Kp, par ? 1 : 0);
-    else im2col_patch_kernel<<<grid, 256, 0, st>>>(images, u, NI, h->in_h, h->in_w, h->cfg.patch, gh, gw, Kp, par ? 1 : 0);
+    im2col_patch_kernel<<<grid, 256, 0, st>>>(images, u, tab, NI, L - 1, h->cfg.patch, Kp, par ? 1 : 0);
     CKL(h, "im2col_patch_kernel");
     GemmCall c = gemm_rows(h, RowOut::F32, u, h->w_patch.as<bf16>(), NI * (L - 1), d, Kp, nullptr, ACT_NONE, nullptr, x);
     c.p.rows_per_batch = L - 1;
@@ -1230,15 +1257,8 @@ static int encode_impl(gitb200_engine* h, const float* images, int B, int frames
     c.p.row_offset = 1;
     TRY(launch_gemm(h, c, st));
     const int gridr = static_cast<int>((Me + 7) / 8);
-    const RaggedImg* tab = h->rg_tab.as<RaggedImg>();
-    if (d == 768 && rg)
-      cls_pos_lnpre_kernel<768, true><<<gridr, 256, 0, st>>>(x, h->cls.as<float>(), pos, h->lnpre_g.as<float>(), h->lnpre_b.as<float>(), static_cast<int>(Me), L, tab);
-    else if (d == 768)
-      cls_pos_lnpre_kernel<768><<<gridr, 256, 0, st>>>(x, h->cls.as<float>(), pos, h->lnpre_g.as<float>(), h->lnpre_b.as<float>(), static_cast<int>(Me), L);
-    else if (rg)
-      cls_pos_lnpre_kernel<1024, true><<<gridr, 256, 0, st>>>(x, h->cls.as<float>(), pos, h->lnpre_g.as<float>(), h->lnpre_b.as<float>(), static_cast<int>(Me), L, tab);
-    else
-      cls_pos_lnpre_kernel<1024><<<gridr, 256, 0, st>>>(x, h->cls.as<float>(), pos, h->lnpre_g.as<float>(), h->lnpre_b.as<float>(), static_cast<int>(Me), L);
+    auto kern = d == 768 ? cls_pos_lnpre_kernel<768> : cls_pos_lnpre_kernel<1024>;
+    kern<<<gridr, 256, 0, st>>>(x, h->cls.as<float>(), pos, h->lnpre_g.as<float>(), h->lnpre_b.as<float>(), static_cast<int>(Me), L, tab);
     CKL(h, "cls_pos_lnpre_kernel");
   }
   const int rows = static_cast<int>(Me);
@@ -1248,7 +1268,7 @@ static int encode_impl(gitb200_engine* h, const float* images, int B, int frames
   attn.B = NI; attn.S = L; attn.H = H;
   attn.q_rs = attn.kv_rs = 3 * d; attn.q_bs = attn.kv_bs = static_cast<long long>(L) * 3 * d;
   attn.o_rs = d * ks; attn.o_bs = static_cast<long long>(L) * attn.o_rs;
-  attn.seq_lens = seq_lens;
+  attn.seq_lens = img_lens(h, ib);
   for (int i = 0; i < h->cfg.enc_layers; ++i) {
     EncLayer& l = h->enc[i];
     TRY(launch_ln(h, ln_operand(h, x, l.ln1g.as<float>(), l.ln1b.as<float>(), 1e-5f, nullptr, hb, rows), d, st));
@@ -1264,13 +1284,13 @@ static int encode_impl(gitb200_engine* h, const float* images, int B, int frames
     LnParams p = ln_operand(h, x, h->lnpost_g.as<float>(), h->lnpost_b.as<float>(), 1e-5f, feats_out, h->feats.as<bf16>(), rows);
     p.remap_B = B; p.remap_F = frames; p.remap_L = L;
     // temporal embeddings only for list inputs (reference layers/decoder.py:846-849; a bare tensor skips them)
-    p.temb = (list_input && h->cfg.num_frames_emb > 0) ? h->temb.as<float>() : nullptr;
+    p.temb = (ib.list_input && h->cfg.num_frames_emb > 0) ? h->temb.as<float>() : nullptr;
     TRY(launch_ln(h, p, d, st));
   }
   h->cur_B = B;
   h->cur_frames = frames;
   h->cur_M = frames * L;
-  h->cur_ragged = rg;
+  h->cur_img = ib;
   return 0;
 }
 
@@ -1363,7 +1383,7 @@ static int image_rows(gitb200_engine* h, float* vproj_out, cudaStream_t st) {
   a.B = B; a.S = M; a.H = h->cfg.dec_heads;
   a.q_rs = a.kv_rs = D; a.q_bs = a.kv_bs = static_cast<long long>(M) * D;
   a.o_rs = D * h->ks(); a.o_bs = static_cast<long long>(M) * a.o_rs;
-  a.seq_lens = h->cur_ragged ? h->rg_lens.as<int>() : nullptr;
+  a.seq_lens = img_lens(h, h->cur_img);
   auto self_attention = [&](int, const void* q, const void* k, const void* v, bf16* ctx) {
     a.q = q; a.k = k; a.v = v; a.out = ctx;
     return launch_self_attention(h, a, h->parity, st);
@@ -1465,7 +1485,7 @@ static int step_layers(gitb200_engine* h, cudaStream_t st, const long long* toke
   da.src_row = src_row; da.ctx = ctx;
   da.B = h->cur_B; da.beam = beam; da.M = h->cur_M; da.T_alloc = h->T_alloc; da.D = D;
   da.state = state;
-  da.img_lens = h->cur_ragged ? h->rg_lens.as<int>() : nullptr;
+  da.img_lens = img_lens(h, h->cur_img);
   da.geom = h->attn_geom;
   da.pdl = pdl;
   auto ln = [&](LnParams p) -> int {
@@ -1502,7 +1522,7 @@ static int step_layers(gitb200_engine* h, cudaStream_t st, const long long* toke
 
 // Decode-attention geometry of the last prefill (dec_attn_geometry) and the step chain's counters.
 static int set_decode_geometry(gitb200_engine* h) {
-  h->attn_geom = dec_attn_geometry(h->cur_M, h->cur_ragged ? h->cur_lens.data() : nullptr, h->cur_B, h->num_sms,
+  h->attn_geom = dec_attn_geometry(h->cur_M, h->cur_img.ragged ? h->cur_img.lens.data() : nullptr, h->cur_B, h->num_sms,
                                    h->cur_B * h->cfg.dec_heads);
   CK(h->chain.ensure(256));
   CK(cudaMemset(h->chain.p, 0, 256));

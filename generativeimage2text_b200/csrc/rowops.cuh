@@ -202,52 +202,6 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const LnParams p) {
   chain_signal(p.chain);
 }
 
-// Patch im2col for the stride==kernel conv (reference layers/CLIP/model.py:224,242):
-// A[(img, py, px)][(c, ky, kx)] = img[c, py*p+ky, px*p+kx], zero-padded to Kp columns, bf16.
-__global__ void im2col_patch_kernel(const float* __restrict__ img, __nv_bfloat16* __restrict__ A, int n_img, int H, int W,
-                                    int p, int gh, int gw, int Kp, int split3) {
-  const long long total = static_cast<long long>(n_img) * gh * gw * (Kp / 8);
-  const int K = 3 * p * p;
-  for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
-       idx += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int kc = static_cast<int>(idx % (Kp / 8));
-    const long long row = idx / (Kp / 8);
-    const int px = static_cast<int>(row % gw);
-    const int py = static_cast<int>((row / gw) % gh);
-    const long long im = row / (gh * gw);
-    float v[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int k = kc * 8 + j;
-      float x = 0.f;
-      if (k < K) {
-        const int c = k / (p * p);
-        const int r = k - c * p * p;
-        const int ky = r / p;
-        const int kx = r - ky * p;
-        x = __ldg(img + ((im * 3 + c) * H + (py * p + ky)) * static_cast<long long>(W) + (px * p + kx));
-      }
-      v[j] = x;
-    }
-    if (split3) {   // parity mode: [hi | lo | hi], 3 x Kp columns
-      uint4 hi, lo;
-      pack_split2(v[0], v[1], hi.x, lo.x);
-      pack_split2(v[2], v[3], hi.y, lo.y);
-      pack_split2(v[4], v[5], hi.z, lo.z);
-      pack_split2(v[6], v[7], hi.w, lo.w);
-      uint4* dst = reinterpret_cast<uint4*>(A + row * 3 * Kp) + kc;
-      dst[0] = hi; dst[Kp / 8] = lo; dst[Kp / 4] = hi;
-      continue;
-    }
-    uint4 o;
-    o.x = pack_bf16(v[0], v[1]);
-    o.y = pack_bf16(v[2], v[3]);
-    o.z = pack_bf16(v[4], v[5]);
-    o.w = pack_bf16(v[6], v[7]);
-    reinterpret_cast<uint4*>(A + row * Kp)[kc] = o;
-  }
-}
-
 // Positional embedding [1 + g0*g0, d] re-sampled to a gh x gw grid for inputs whose size differs from the resolution the
 // embedding was built for (reference layers/CLIP/model.py:245-251): CLS row copied, grid rows =
 // F.interpolate(mode='bicubic', align_corners=False), i.e. source coordinate (o + 0.5) * in / out - 0.5, Keys cubic with
@@ -299,19 +253,19 @@ pos_embed_bicubic_kernel(const float* __restrict__ pos, float* __restrict__ out,
   }
 }
 
-// Ragged batches (gitb200_set_image_sizes): image b of a call is [3, h, w] at src_off floats into the packed pixels, has a
-// gh x gw patch grid and L = gh * gw + 1 valid tokens in its slot of L_max rows, and reads its positional embedding from
-// row pos_row of the call's table of re-sampled embeddings.
+// One encoded image of a call (gitb200.cu ImageBatch): [3, h, w] at src_off floats into the call's pixels, a gh x gw patch
+// grid and L = gh * gw + 1 valid tokens in its slot of L_max rows; its positional embedding starts at row pos_row of the
+// call's positional table.
 struct RaggedImg {
   long long src_off;
   int h, w, gh, gw, L, pos_row;
 };
 
-// im2col_patch_kernel for a ragged batch: every image owns n_slot = L_max - 1 rows of A (uniform row map for the patch
-// GEMM); rows past its own gh * gw patches are zero.
-__global__ void im2col_patch_ragged_kernel(const float* __restrict__ img, __nv_bfloat16* __restrict__ A,
-                                           const RaggedImg* __restrict__ tab, int n_img, int n_slot, int p, int Kp,
-                                           int split3) {
+// Patch im2col for the stride==kernel conv (reference layers/CLIP/model.py:224,242):
+// A[(img, py, px)][(c, ky, kx)] = img[c, py*p+ky, px*p+kx], zero-padded to Kp columns, bf16.  Every image owns
+// n_slot = L_max - 1 rows of A (one row map for the patch GEMM); rows past its own gh * gw patches are zero.
+__global__ void im2col_patch_kernel(const float* __restrict__ img, __nv_bfloat16* __restrict__ A,
+                                    const RaggedImg* __restrict__ tab, int n_img, int n_slot, int p, int Kp, int split3) {
   const long long total = static_cast<long long>(n_img) * n_slot * (Kp / 8);
   const int K = 3 * p * p;
   for (long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; idx < total;
@@ -342,7 +296,7 @@ __global__ void im2col_patch_ragged_kernel(const float* __restrict__ img, __nv_b
 #pragma unroll
       for (int j = 0; j < 8; ++j) v[j] = 0.f;
     }
-    if (split3) {
+    if (split3) {   // parity mode: [hi | lo | hi], 3 x Kp columns
       uint4 hi, lo;
       pack_split2(v[0], v[1], hi.x, lo.x);
       pack_split2(v[2], v[3], hi.y, lo.y);
@@ -363,28 +317,26 @@ __global__ void im2col_patch_ragged_kernel(const float* __restrict__ img, __nv_b
 
 // x[img, l] = ln_pre((l == 0 ? class_embedding : patch_out[img, l]) + positional_embedding[l])
 // in place on the fp32 residual stream (reference layers/CLIP/model.py:254-257).
-// kRagged: L is the slot length L_max; image b takes its positional rows from pos + tab[b].pos_row and its rows past
-// tab[b].L are set to zero (finite padding: no valid row ever reads them).
-template <int D, bool kRagged = false>
+// L is the slot length L_max: image b takes its positional rows from pos + tab[b].pos_row and its rows past tab[b].L are
+// set to zero (finite padding: no valid row ever reads them).
+template <int D>
 __global__ void __launch_bounds__(256)
 cls_pos_lnpre_kernel(float* __restrict__ x, const float* __restrict__ cls, const float* __restrict__ pos,
                      const float* __restrict__ gamma, const float* __restrict__ beta, int rows, int L,
-                     const RaggedImg* __restrict__ tab = nullptr) {
+                     const RaggedImg* __restrict__ tab) {
   constexpr int NV = D / 128;
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= rows) return;
   const int lane = threadIdx.x & 31;
   const int l = row % L;
-  if constexpr (kRagged) {
-    const RaggedImg& e = tab[row / L];
-    if (l >= e.L) {
-      float4* op = reinterpret_cast<float4*>(x + static_cast<long long>(row) * D);
+  const RaggedImg& e = tab[row / L];
+  if (l >= e.L) {
+    float4* op = reinterpret_cast<float4*>(x + static_cast<long long>(row) * D);
 #pragma unroll
-      for (int i = 0; i < NV; ++i) op[i * 32 + lane] = make_float4(0.f, 0.f, 0.f, 0.f);
-      return;
-    }
-    pos += static_cast<long long>(e.pos_row) * D;
+    for (int i = 0; i < NV; ++i) op[i * 32 + lane] = make_float4(0.f, 0.f, 0.f, 0.f);
+    return;
   }
+  pos += static_cast<long long>(e.pos_row) * D;
   float4 v[NV];
   const float4* src = (l == 0) ? reinterpret_cast<const float4*>(cls)
                                : reinterpret_cast<const float4*>(x + static_cast<long long>(row) * D);

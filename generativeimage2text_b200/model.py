@@ -8,6 +8,7 @@ its `forward(batch)` accepts the reference's batch dict and returns `{'predictio
 token ids come out of libgitb200.so (hand-written sm_90a kernels).  PyTorch only owns the parameter
 storage, the CUDA stream and the output tensors.
 """
+import collections
 import ctypes
 import warnings
 
@@ -159,6 +160,11 @@ def greedy_width(pred, eos):
     return int(hit[0]) + 1 if hit.numel() else pred.shape[1]
 
 
+# One call's images as the engine takes them (GitB200CaptioningModel._image_batch): x = the pixels on the device, B images,
+# frames (0: a bare tensor), sizes = [(H_b, W_b)] of a ragged batch or None, tokens = image tokens L_b of each image.
+_Images = collections.namedtuple('_Images', 'x B frames sizes tokens')
+
+
 class _Group(object):
     """Batches submitted one by one that share ONE engine launch (dynamic batching): one encoder pass over all their
     images and one decode chain over all their rows.  The decode chain is ~45 latency-bound kernels per step whose
@@ -169,9 +175,9 @@ class _Group(object):
         self.images, self.rows = [], []
         self.pending, self.out = None, None
 
-    def add(self, image, rows):
-        self.images.append(image)
-        self.rows.append(rows)
+    def add(self, img):
+        self.images.append(img)
+        self.rows.append(img.B)
         return len(self.rows) - 1
 
     def launch(self):
@@ -180,15 +186,12 @@ class _Group(object):
         m = self.model
         if m._open_group is self:
             m._open_group = None
-        first = self.images[0]
-        if len(self.images) == 1:
-            cat = first
-        elif isinstance(first, (list, tuple)):
-            cat = [torch.cat([im[f] for im in self.images], dim=0) for f in range(len(first))]
-        else:
-            cat = torch.cat(self.images, dim=0)
+        img = self.images[0]
+        if len(self.images) > 1:   # along the batch axis: [frames, B, 3, H, W] of several frames, else [B, 3, H, W]
+            x = torch.cat([im.x for im in self.images], dim=1 if img.frames > 1 else 0)
+            img = img._replace(x=x, B=sum(self.rows), tokens=img.tokens[:1] * sum(self.rows))
         self.images = None
-        self.pending = m.submit({'image': cat}, depth=self.depth)
+        self.pending = m.submit({'image': img}, depth=self.depth)
 
     def result(self):
         if self.out is None:
@@ -418,60 +421,58 @@ class GitB200CaptioningModel(nn.Module):
         raise TypeError('model.decoder must be an AutoRegressiveBeamSearch, TrieAutoRegressiveBeamSearch or GeneratorWithBeamSearch '
                         'of this package')
 
-    @staticmethod
-    def _is_ragged(image):
-        """A list of 3-D [3, H_b, W_b] tensors = B single images of their own sizes (a list of 4-D tensors = video frames)."""
-        if not isinstance(image, (list, tuple)) or not image:
-            return False
-        dims = [im.dim() for im in image]
-        if 3 in dims and any(n != 3 for n in dims):
-            raise ValueError('a ragged batch is a list of [3, H, W] images; it cannot be mixed with [B, 3, H, W] frames')
-        return dims[0] == 3
-
-    def _pack_ragged(self, image):
-        """List of [3, H_b, W_b] images -> (the B images back to back as one fp32 vector on the device, B, [(H_b, W_b)])."""
-        enc = ENCODER_CFG[self.param.get('image_encoder_type', 'CLIPViT_B_16')]
-        sizes = []
-        for b, im in enumerate(image):
-            if im.shape[0] != 3:
-                raise ValueError('image %d of a ragged batch must be [3, H, W] (got %s)' % (b, tuple(im.shape)))
-            if im.shape[1] < enc['patch'] or im.shape[2] < enc['patch']:
-                raise ValueError('image %d (%s) is smaller than one patch' % (b, tuple(im.shape[1:])))
-            sizes.append((int(im.shape[1]), int(im.shape[2])))
-        dev = self._device()
-        x = torch.cat([im.to(device=dev, dtype=torch.float32, non_blocking=True).reshape(-1) for im in image])
-        return x, len(sizes), sizes
-
-    def _image_tokens(self, sizes):
-        """Image tokens L_b of each (H_b, W_b): the patch grid plus the class token."""
+    def _image_batch(self, image):
+        """Checks one call's 'image' argument and puts its pixels on the device as the engine reads them -> _Images.
+        A list of [3, H_b, W_b] tensors is a ragged batch (B single images of their own sizes, back to back), a list of
+        [B, 3, H, W] tensors is video frames ([frames, B, 3, H, W]) and a bare [B, 3, H, W] tensor has frames = 0 (no
+        temporal embedding)."""
         p = ENCODER_CFG[self.param.get('image_encoder_type', 'CLIPViT_B_16')]['patch']
-        return [(h // p) * (w // p) + 1 for h, w in sizes]
-
-    @staticmethod
-    def _sizes_arg(sizes):
-        """(int32 [n][2] host array of the sizes, n) for gitb200_set_image_sizes."""
-        return (ctypes.c_int32 * (2 * len(sizes)))(*[v for hw in sizes for v in hw]), len(sizes)
-
-    def _pack_images(self, image):
-        """-> (fp32 contiguous [frames*B,3,S,S] on device, B, frames) ; frames = 0 for a bare tensor."""
         dev = self._device()
+
+        def to_dev(t):
+            return t.to(device=dev, dtype=torch.float32, non_blocking=True)
+        frames = 0
         if isinstance(image, (list, tuple)):
+            if not image:
+                raise ValueError('an image list must not be empty')
+            dims = [im.dim() for im in image]
+            if 3 in dims and any(n != 3 for n in dims):
+                raise ValueError('a ragged batch is a list of [3, H, W] images; it cannot be mixed with [B, 3, H, W] frames')
+            if dims[0] == 3:
+                sizes = []
+                for b, im in enumerate(image):
+                    if im.shape[0] != 3:
+                        raise ValueError('image %d of a ragged batch must be [3, H, W] (got %s)' % (b, tuple(im.shape)))
+                    if im.shape[1] < p or im.shape[2] < p:
+                        raise ValueError('image %d (%s) is smaller than one patch' % (b, tuple(im.shape[1:])))
+                    sizes.append((int(im.shape[1]), int(im.shape[2])))
+                x = torch.cat([to_dev(im).reshape(-1) for im in image])
+                return _Images(x, len(sizes), 0, sizes, [(h // p) * (w // p) + 1 for h, w in sizes])
             frames = len(image)
-            ims = [im.to(device=dev, dtype=torch.float32, non_blocking=True) for im in image]
-            B = ims[0].shape[0]
+            ims = [to_dev(im) for im in image]
             if any(im.shape != ims[0].shape for im in ims):
                 raise ValueError('all frames of a batch must share one size')
             x = ims[0].contiguous() if frames == 1 else torch.stack(ims, dim=0).contiguous()
         else:
-            frames = 0
-            x = image.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
-            B = x.shape[0]
+            x = to_dev(image).contiguous()
         if x.dim() != (4 if frames <= 1 else 5) or x.shape[-3] != 3:
             raise ValueError('images must be [B, 3, H, W] tensors (got %s)' % (tuple(x.shape),))
-        enc = ENCODER_CFG[self.param.get('image_encoder_type', 'CLIPViT_B_16')]
-        if x.shape[-2] < enc['patch'] or x.shape[-1] < enc['patch']:
-            raise ValueError('input %s is smaller than one patch' % (tuple(x.shape[-2:]),))
-        return x, B, frames
+        H, W = int(x.shape[-2]), int(x.shape[-1])
+        if H < p or W < p:
+            raise ValueError('input %s is smaller than one patch' % ((H, W),))
+        B = int(x.shape[-4])
+        return _Images(x, B, frames, None, [(H // p) * (W // p) + 1] * B)
+
+    @staticmethod
+    def _set_image_sizes(lib, eng, img):
+        """Hands the sizes of `img` to engine `eng`: every image's own size for the next call only, or the one size of
+        them all (sticky; inputs of another size than test_crop_size, reference inference.py:29-64, get the positional
+        embedding re-sampled to their patch grid, reference layers/CLIP/model.py:245-251)."""
+        if img.sizes is None:
+            _lib.check(lib.gitb200_set_input_size(eng, int(img.x.shape[-2]), int(img.x.shape[-1])), eng, 'set_input_size')
+        else:
+            hw = (ctypes.c_int32 * (2 * img.B))(*[v for s in img.sizes for v in s])
+            _lib.check(lib.gitb200_set_image_sizes(eng, hw, img.B), eng, 'set_image_sizes')
 
     # ---------------------------------------------------------------- the reference surface
     @torch.no_grad()
@@ -508,10 +509,14 @@ class GitB200CaptioningModel(nn.Module):
             raise NotImplementedError("'context' batches are not produced by the reference inference path")
         search_param = dict(search_param or {})
         constrained = bool(search_param) or isinstance(self.decoder, TrieAutoRegressiveBeamSearch)
-        ragged = self._is_ragged(batch['image'])     # a ragged batch is launched on its own (never coalesced)
-        if (int(coalesce) > 1 and not ragged and slot is None and not _caller_stream and forced_tokens is None and not return_step_logits
+        image = batch['image']
+        # (copies / casts, if any, run on the caller's stream; a coalesced group hands over its images as one _Images)
+        img = image if isinstance(image, _Images) else self._image_batch(image)
+        x, B, frames = img.x, img.B, img.frames
+        # a ragged batch is launched on its own (never coalesced)
+        if (int(coalesce) > 1 and img.sizes is None and slot is None and not _caller_stream and forced_tokens is None and not return_step_logits
                 and 'prefix' not in batch and 'prefix_len' not in batch and not constrained):
-            return self._submit_coalesced(batch['image'], depth, int(coalesce))
+            return self._submit_coalesced(img, depth, int(coalesce))
         if self._open_group is not None:
             self._open_group.launch()         # keep the submission order
         if slot is None:
@@ -525,12 +530,6 @@ class GitB200CaptioningModel(nn.Module):
         eng = sl['engine']
         dev = self._device()
         cur = torch.cuda.current_stream(dev)
-        # (copies / casts, if any, run on the caller's stream)
-        if ragged:
-            x, B, sizes = self._pack_ragged(batch['image'])
-            frames = 0
-        else:
-            x, B, frames = self._pack_images(batch['image'])
         if _caller_stream:
             stream = cur                      # synchronous path: the caller's stream (stream 0 -> engine-owned stream)
         else:
@@ -578,13 +577,7 @@ class GitB200CaptioningModel(nn.Module):
         for t in (x, prefix, forced, row_prefix, row_lens_dev, uniforms):
             if t is not None and stream is not cur:
                 t.record_stream(stream)
-        # inputs of another size than test_crop_size (MinMaxResizeForTest, reference inference.py:29-64): the engine
-        # re-samples the positional embedding to their patch grid (reference layers/CLIP/model.py:245-251)
-        # (a ragged batch: every image's own size, for this call only)
-        if ragged:
-            _lib.check(lib.gitb200_set_image_sizes(eng, *self._sizes_arg(sizes)), eng, 'set_image_sizes')
-        else:
-            _lib.check(lib.gitb200_set_input_size(eng, int(x.shape[-2]), int(x.shape[-1])), eng, 'set_input_size')
+        self._set_image_sizes(lib, eng, img)
         if row_prefix is not None:
             _lib.check(lib.gitb200_set_row_prefixes(eng, row_prefix.data_ptr(), B, int(row_prefix.shape[1]), row_lens_dev.data_ptr()),
                        eng, 'set_row_prefixes')
@@ -603,25 +596,16 @@ class GitB200CaptioningModel(nn.Module):
 
     # ---------------------------------------------------------------- caption scoring
     def _score_args(self, batch):
-        """Host-side checks of a score() batch (before any engine is touched) -> (image, B, tokens, need_predict, image_index),
-        the last three as CPU tensors."""
+        """Host-side checks of a score() batch (before any engine is touched) -> (_Images, B, tokens, need_predict,
+        image_index), the last three as CPU tensors."""
         for key in ('context', 'bi_valid_mask_caption'):
             if key in batch:
                 raise NotImplementedError("score(): %r batches are not supported" % key)
         for key in ('image', 'caption_tokens', 'need_predict'):
             if key not in batch:
                 raise ValueError("score(): batch needs %r" % key)
-        image = batch['image']
-        if self._is_ragged(image):
-            B = len(image)
-        elif isinstance(image, (list, tuple)):
-            if not image or image[0].dim() != 4:
-                raise ValueError('score(): video frames must be a list of [B, 3, H, W] tensors')
-            B = int(image[0].shape[0])
-        else:
-            if image.dim() != 4:
-                raise ValueError("score(): 'image' must be [B, 3, H, W] (got %s)" % (tuple(image.shape),))
-            B = int(image.shape[0])
+        img = self._image_batch(batch['image'])
+        B = img.B
         tokens = torch.as_tensor(batch['caption_tokens']).detach().cpu()
         need = torch.as_tensor(batch['need_predict']).detach().cpu()
         if tokens.dim() != 2 or tokens.dtype.is_floating_point:
@@ -648,7 +632,7 @@ class GitB200CaptioningModel(nn.Module):
             raise ValueError("score(): %d captions for %d images need an 'image_index'" % (N, B))
         if not bool(((need[:, 1:] == 1) & (tokens[:, 1:] != 0)).any()):
             raise ValueError('score(): no position to predict (need_predict == 1 with a non-zero target)')
-        return image, B, tokens.long(), need.long(), index
+        return img, B, tokens.long(), need.long(), index
 
     @torch.no_grad()
     def score(self, batch):
@@ -662,31 +646,22 @@ class GitB200CaptioningModel(nn.Module):
                  'vl_l_loss': fp32 scalar = the reference's SmoothLabelCrossEntropyLoss (eps 0.1) over the positions with
                  need_predict[n, t+1] == 1 and a non-zero target}.
         Captions of one image share its encoder pass.  The arguments are checked on the host (token ids, shapes, indices)."""
-        image, B, tokens, need, index = self._score_args(batch)
+        img, _, tokens, need, index = self._score_args(batch)
         N, T = tokens.shape
-        ragged = self._is_ragged(image)
         lib, _ = self._ensure_engine(0)
         sl = self._slots[0]
         if sl['pending'] is not None:
             sl['pending'].result()
         eng = sl['engine']
         dev = self._device()
-        if ragged:
-            x, B, sizes = self._pack_ragged(image)
-            frames = 0
-        else:
-            x, B, frames = self._pack_images(image)
         tok_d = tokens.to(dev).contiguous()
         need_d = need.to(dev).contiguous()
         idx_d = index.to(device=dev, dtype=torch.int32).contiguous() if index is not None else None
         lp = torch.empty((N, T - 1), dtype=torch.float32, device=dev)
         loss = torch.empty((1,), dtype=torch.float32, device=dev)
-        if ragged:
-            _lib.check(lib.gitb200_set_image_sizes(eng, *self._sizes_arg(sizes)), eng, 'set_image_sizes')
-        else:
-            _lib.check(lib.gitb200_set_input_size(eng, int(x.shape[-2]), int(x.shape[-1])), eng, 'set_input_size')
+        self._set_image_sizes(lib, eng, img)
         stream = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(lib.gitb200_score(eng, x.data_ptr(), B, frames, tok_d.data_ptr(), need_d.data_ptr(),
+        _lib.check(lib.gitb200_score(eng, img.x.data_ptr(), img.B, img.frames, tok_d.data_ptr(), need_d.data_ptr(),
                                      idx_d.data_ptr() if idx_d is not None else None, N, T, lp.data_ptr(), loss.data_ptr(),
                                      stream), eng, 'score')
         return {'token_logprobs': lp, 'vl_l_loss': loss[0]}
@@ -733,30 +708,15 @@ class GitB200CaptioningModel(nn.Module):
             _lib.check(lib.gitb200_set_trie(eng, arr(begin), arr(tok), arr(child), len(begin) - 1, len(tok)), eng, 'set_trie')
         sl['trie_key'] = key
 
-    def _submit_coalesced(self, image, depth, want):
-        dev = self._device()
-        if dev.type != 'cuda':
-            raise RuntimeError('the gitb200 engine runs on CUDA devices only (sm_90a); call model.cuda() first. '
-                               'There is no CPU path.')
-
-        def to_dev(t):
-            return t.to(device=dev, dtype=torch.float32, non_blocking=True)
-        if isinstance(image, (list, tuple)):
-            image = [to_dev(im) for im in image]
-            key = ('list', len(image)) + tuple(tuple(im.shape[1:]) for im in image)
-            rows = image[0].shape[0]
-        else:
-            image = to_dev(image)
-            key = ('tensor',) + tuple(image.shape[1:])
-            rows = image.shape[0]
-        key = key + (id(self.decoder), depth, want)
+    def _submit_coalesced(self, img, depth, want):
+        key = (img.frames,) + tuple(img.x.shape[-3:]) + (id(self.decoder), depth, want)
         g = self._open_group
         if g is not None and g.key != key:
             g.launch()
             g = None
         if g is None:
             g = self._open_group = _Group(self, key, depth, want)
-        member = _Member(g, g.add(image, rows))
+        member = _Member(g, g.add(img))
         if len(g.rows) >= want:
             g.launch()
         return member
@@ -810,38 +770,31 @@ class GitB200CaptioningModel(nn.Module):
         """Image features as the decoder sees them: [B, frames*L, d] fp32 (reference layers/decoder.py:846-857); for a ragged
         list of [3, H_b, W_b] images, a list of [1, L_b, d] (image b alone, as `encode_image(image[b][None])` gives it)."""
         lib, stream = self._ensure_engine()
-        enc = ENCODER_CFG[self.param.get('image_encoder_type', 'CLIPViT_B_16')]
-        if self._is_ragged(image):
-            x, B, sizes = self._pack_ragged(image)
-            lens = self._image_tokens(sizes)
-            feats = torch.empty((B, max(lens), enc['width']), dtype=torch.float32, device=x.device)
-            self._m_tokens = max(lens)
-            _lib.check(lib.gitb200_set_image_sizes(self._engine, *self._sizes_arg(sizes)), self._engine, 'set_image_sizes')
-            _lib.check(lib.gitb200_encode(self._engine, x.data_ptr(), B, 0, feats.data_ptr(), stream), self._engine, 'encode')
-            return [feats[b:b + 1, :n] for b, n in enumerate(lens)]
-        x, B, frames = self._pack_images(image)
-        L = (x.shape[-2] // enc['patch']) * (x.shape[-1] // enc['patch']) + 1
-        _lib.check(lib.gitb200_set_input_size(self._engine, int(x.shape[-2]), int(x.shape[-1])), self._engine, 'set_input_size')
-        nf = max(frames, 1)
-        if frames and self.num_image_with_embedding:
-            nf = min(nf, self.num_image_with_embedding)
-        feats = torch.empty((B, nf * L, enc['width']), dtype=torch.float32, device=x.device)
-        self._m_tokens = nf * L
-        _lib.check(lib.gitb200_encode(self._engine, x.data_ptr(), B, frames, feats.data_ptr(), stream), self._engine,
-                   'encode')
+        img = self._image_batch(image)
+        if img.sizes is not None:
+            M = max(img.tokens)
+        else:
+            nf = max(img.frames, 1)
+            if img.frames and self.num_image_with_embedding:
+                nf = min(nf, self.num_image_with_embedding)
+            M = nf * img.tokens[0]
+        width = ENCODER_CFG[self.param.get('image_encoder_type', 'CLIPViT_B_16')]['width']
+        feats = torch.empty((img.B, M, width), dtype=torch.float32, device=img.x.device)
+        self._m_tokens = M
+        self._set_image_sizes(lib, self._engine, img)
+        _lib.check(lib.gitb200_encode(self._engine, img.x.data_ptr(), img.B, img.frames, feats.data_ptr(), stream),
+                   self._engine, 'encode')
+        if img.sizes is not None:
+            return [feats[b:b + 1, :n] for b, n in enumerate(img.tokens)]
         return feats
 
     @torch.no_grad()
     def prefill(self, batch_size, beam=1):
         """visual_projection output [B, M, 768] fp32 after the last encode_image; fills the image K/V cache."""
         lib, stream = self._ensure_engine()
-        M = self._last_M(batch_size)
-        out = torch.empty((batch_size, M, HIDDEN), dtype=torch.float32, device=self._device())
+        out = torch.empty((batch_size, self._m_tokens, HIDDEN), dtype=torch.float32, device=self._device())
         _lib.check(lib.gitb200_prefill(self._engine, batch_size, beam, out.data_ptr(), stream), self._engine, 'prefill')
         return out
-
-    def _last_M(self, batch_size):
-        return self._m_tokens
 
     @torch.no_grad()
     def decoding_step(self, tokens, pos, beam_idx=None):

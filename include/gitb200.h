@@ -345,9 +345,9 @@ int gitb200_preproc_coeffs(int in_size, int out_size, int32_t* ksize_out, int32_
  *                 in the encoder's order f*batch + b (L: tokens per image; a ragged batch's slot length L_max);
  *   "enc_feats"   the features as the prefill's GEMM operand: bf16 [batch*frames*L][width], or [hi | lo | hi] rows of
  *                 3*width in parity mode (hi = bf16(f), lo = bf16(f - hi)); rows in the output order b*frames*L + f*L + l;
- *   "pos_interp"  fp32 [rows][width]: the positional table the encode re-sampled, 1 + gh*gw rows for one input size, one
- *                 table per distinct patch grid of a ragged batch in order of first appearance (the model's own grid copied);
- *                 0 bytes when the encode used the stored table.
+ *   "pos_interp"  fp32 [rows][width]: the positional table the encode made, one block of 1 + gh*gw rows per distinct patch
+ *                 grid of its images in order of first appearance (the model's own grid copied, any other re-sampled);
+ *                 0 bytes when every image had the model's grid and the encode used the stored table.
  * Beam search bookkeeping, current side of each ping-pong:
  *   "src_row"     int32 [rows][T_alloc]: the text-K/V indirection table the next beam step reads (position j of logical
  *                 row r is held by physical row src_row[r][j]); after a beam generate or the raw decode_step API;

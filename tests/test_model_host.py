@@ -39,11 +39,17 @@ class _FakeModel:
         return _FakePending(self.out)
 
 
+def _rec(x, frames=0):
+    """The images of one batch as GitB200CaptioningModel._image_batch records them (x: [B, 3, H, W] or [frames, B, 3, H, W])."""
+    B = int(x.shape[-4])
+    return M._Images(x, B, frames, None, [1] * B)
+
+
 def _greedy():
     return M.AutoRegressiveBeamSearch(EOS, max_steps=6, beam_size=1, per_node_beam_size=1, fix_missing_prefix=True)
 
 
-def test_members_get_their_own_rows_widths_and_the_empty_caption_exit():
+def test_members_of_coalesced_image_records_get_their_own_rows_widths_and_the_empty_caption_exit():
     toks = torch.tensor([
         [101, 11, 12, 13, 14, 15],      # batch 0 (2 rows): never finishes -> full width
         [101, 21, EOS, EOS, EOS, EOS],
@@ -56,10 +62,12 @@ def test_members_get_their_own_rows_widths_and_the_empty_caption_exit():
     g = M._Group(fm, key=('k',), depth=2, want=3)
     fm._open_group = g
     imgs = [torch.zeros(2, 3, 4, 4), torch.ones(2, 3, 4, 4), torch.full((1, 3, 4, 4), 2.0)]
-    members = [M._Member(g, g.add(im, im.shape[0])) for im in imgs]
+    members = [M._Member(g, g.add(_rec(im))) for im in imgs]
     g.launch()
     assert fm._open_group is None and len(fm.launched) == 1
-    assert fm.launched[0].shape == (5, 3, 4, 4) and float(fm.launched[0][2:4].mean()) == 1.0     # concatenated in order
+    cat = fm.launched[0]
+    assert cat.B == 5 and cat.frames == 0
+    assert cat.x.shape == (5, 3, 4, 4) and float(cat.x[2:4].mean()) == 1.0                       # concatenated in order
     g.launch()                                                                                   # idempotent
     assert len(fm.launched) == 1
     a = members[0].result()
@@ -74,19 +82,19 @@ def test_members_get_their_own_rows_widths_and_the_empty_caption_exit():
     assert members[1].result() is b                                                              # cached
 
 
-def test_list_inputs_are_concatenated_frame_by_frame_and_beam_results_are_sliced():
+def test_video_records_are_concatenated_along_the_batch_axis_and_beam_results_are_sliced():
     beam = M.GeneratorWithBeamSearch(EOS, max_steps=4, beam_size=4, length_penalty=0.6)
     toks = torch.arange(12).reshape(3, 4)
     lps = torch.tensor([[-0.1], [-0.2], [-0.3]])
     fm = _FakeModel(beam, {'predictions': toks, 'logprobs': lps})
     g = M._Group(fm, key=('k',), depth=2, want=2)
-    a = [torch.zeros(1, 3, 2, 2), torch.zeros(1, 3, 2, 2) + 1]          # 2 frames, 1 image
-    b = [torch.zeros(2, 3, 2, 2) + 5, torch.zeros(2, 3, 2, 2) + 6]      # 2 frames, 2 images
-    ma, mb = M._Member(g, g.add(a, 1)), M._Member(g, g.add(b, 2))
+    a = torch.stack([torch.zeros(1, 3, 2, 2), torch.zeros(1, 3, 2, 2) + 1])          # 2 frames, 1 image
+    b = torch.stack([torch.zeros(2, 3, 2, 2) + 5, torch.zeros(2, 3, 2, 2) + 6])      # 2 frames, 2 images
+    ma, mb = M._Member(g, g.add(_rec(a, 2))), M._Member(g, g.add(_rec(b, 2)))
     ra = ma.result()                                                   # asking for a result launches the group
     cat = fm.launched[0]
-    assert isinstance(cat, list) and len(cat) == 2 and cat[0].shape == (3, 3, 2, 2)
-    assert cat[0][:, 0, 0, 0].tolist() == [0.0, 5.0, 5.0] and cat[1][:, 0, 0, 0].tolist() == [1.0, 6.0, 6.0]
+    assert cat.frames == 2 and cat.B == 3 and cat.x.shape == (2, 3, 3, 2, 2)
+    assert cat.x[0][:, 0, 0, 0].tolist() == [0.0, 5.0, 5.0] and cat.x[1][:, 0, 0, 0].tolist() == [1.0, 6.0, 6.0]
     assert ra['predictions'].tolist() == toks[0:1].tolist() and tuple(ra['logprobs'].shape) == (1, 1)
     assert mb.result()['predictions'].tolist() == toks[1:3].tolist()
 

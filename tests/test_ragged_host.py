@@ -32,34 +32,41 @@ def _imgs(hws):
     return [torch.full((3, h, w), float(b)) for b, (h, w) in enumerate(hws)]
 
 
-def test_lists_of_3d_images_are_ragged_and_frames_keep_their_meaning():
-    assert M.GitB200CaptioningModel._is_ragged(_imgs(HWS))
-    assert not M.GitB200CaptioningModel._is_ragged([torch.zeros(2, 3, 16, 16), torch.zeros(2, 3, 16, 16)])   # video frames
-    assert not M.GitB200CaptioningModel._is_ragged(torch.zeros(2, 3, 16, 16))
+def test_image_batch_reads_lists_of_3d_images_as_ragged_and_frames_keep_their_meaning():
+    m = M.get_git_model(Tok(), RATIO)
+    assert m._image_batch(_imgs(HWS)).sizes == HWS
+    video = m._image_batch([torch.zeros(2, 3, 16, 16), torch.zeros(2, 3, 16, 16)])   # video frames
+    assert video.sizes is None and (video.B, video.frames) == (2, 2)
+    bare = m._image_batch(torch.zeros(2, 3, 16, 16))
+    assert bare.sizes is None and (bare.B, bare.frames) == (2, 0)
     with pytest.raises(ValueError, match='mixed'):
-        M.GitB200CaptioningModel._is_ragged([torch.zeros(3, 16, 16), torch.zeros(1, 3, 16, 16)])
+        m._image_batch([torch.zeros(3, 16, 16), torch.zeros(1, 3, 16, 16)])
 
 
-def test_ragged_validation_errors():
+def test_image_batch_ragged_validation_errors():
     m = M.get_git_model(Tok(), RATIO)
     with pytest.raises(ValueError, match=r'\[3, H, W\]'):
-        m._pack_ragged([torch.zeros(3, 32, 32), torch.zeros(4, 32, 32)])
+        m._image_batch([torch.zeros(3, 32, 32), torch.zeros(4, 32, 32)])
     with pytest.raises(ValueError, match='smaller than one patch'):
-        m._pack_ragged([torch.zeros(3, 32, 32), torch.zeros(3, 15, 64)])
+        m._image_batch([torch.zeros(3, 32, 32), torch.zeros(3, 15, 64)])
 
 
-def test_packing_offsets_and_token_counts():
+def test_image_batch_packing_offsets_token_counts_and_size_array():
     m = M.get_git_model(Tok(), RATIO)
     imgs = _imgs(HWS)
-    x, B, sizes = m._pack_ragged(imgs)
-    assert B == 4 and sizes == HWS
+    img = m._image_batch(imgs)
+    x = img.x
+    assert img.B == 4 and img.frames == 0 and img.sizes == HWS
     assert x.dim() == 1 and x.dtype == torch.float32 and x.numel() == sum(3 * h * w for h, w in HWS)
     off = 0
     for b, (h, w) in enumerate(HWS):                       # image b: [3, h, w] back to back after the ones before it
         assert torch.equal(x[off:off + 3 * h * w].view(3, h, w), imgs[b])
         off += 3 * h * w
-    assert m._image_tokens(sizes) == [131, 131, 101, 141]     # grids 10x13, 13x10, 10x10, 10x14 + the class token
-    arr, n = m._sizes_arg(sizes)
+    assert img.tokens == [131, 131, 101, 141]                 # grids 10x13, 13x10, 10x10, 10x14 + the class token
+    stub = _StubLib()
+    m._set_image_sizes(stub, 'eng', img)
+    [(name, (eng, arr, n))] = stub.calls
+    assert name == 'gitb200_set_image_sizes' and eng == 'eng'
     assert n == 4 and list(arr) == [160, 208, 208, 160, 160, 160, 160, 224]
 
 
