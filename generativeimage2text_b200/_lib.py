@@ -5,7 +5,7 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, 'libgitb200.so')
-ABI_VERSION = 10
+ABI_VERSION = 11
 
 c_void_p, c_int, c_int64, c_float, c_char_p = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_char_p
 c_ll = ctypes.c_longlong
@@ -68,6 +68,7 @@ SIGNATURES = {
     'gitb200_set_row_prefixes': (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
     'gitb200_set_trie': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int]),
     'gitb200_set_sampling': (c_int, [c_void_p, c_void_p, c_int, c_int, c_float]),
+    'gitb200_set_beam_sampling': (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_float]),
     'gitb200_launch_count': (c_int64, [c_void_p]),
     'gitb200_set_option': (c_int, [c_void_p, c_char_p, c_int64]),
     'gitb200_preproc_create': (c_int, [c_int, ctypes.POINTER(c_void_p)]),
@@ -102,6 +103,8 @@ SIGNATURES = {
     'gitb200_op_decode_attention': (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                             c_void_p, c_int, c_int, c_int, ctypes.POINTER(ctypes.c_int32), c_int, c_int,
                                             c_int, c_int, c_int, c_void_p]),
+    'gitb200_op_beam_sample': (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_float, c_int, c_float, c_void_p,
+                                       c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

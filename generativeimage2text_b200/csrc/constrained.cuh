@@ -52,6 +52,59 @@ __device__ __forceinline__ float block_reduce_sum(float v, float* sh) {
   return r;
 }
 
+// Block max of an int (every thread gets it).
+__device__ __forceinline__ int block_reduce_max_int(int v, int* sh) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, o));
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+  __syncthreads();
+  int r = sh[0];
+#pragma unroll
+  for (int w = 1; w < 8; ++w) r = max(r, sh[w]);
+  __syncthreads();
+  return r;
+}
+
+// The index-order inverse-CDF lookup of the sampling kernels (a 256-thread CTA per row): thread t owns the contiguous
+// indices [i0, i1) and `mass_t` is the sum of mass(i) over them in index order.  The target is u * total, total = the
+// thread masses summed in thread order (warp scans, then the 8 warp totals in order).  The owner of the interval
+// [lo, hi) that holds the target walks its indices to the first one whose running mass exceeds it; a target at or beyond
+// the total (u -> 1 and rounding) falls to the last thread, whose walk ends at its last index.  Rounding can make two
+// adjacent threads claim the target (lo is hi - mass_t, not the previous thread's hi): the higher index wins.  Returns
+// the index (every thread), or -1 when no thread claims the target; *total_out = total.
+template <class Mass>
+__device__ __forceinline__ int inverse_cdf_index(float mass_t, float u, int i0, int i1, Mass mass, float* sh_scan, int* sh_pick,
+                                                 float* total_out) {
+  const int tid = threadIdx.x;
+  float inc = mass_t;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float up = __shfl_up_sync(0xffffffffu, inc, o);
+    if ((tid & 31) >= o) inc += up;
+  }
+  if ((tid & 31) == 31) sh_scan[tid >> 5] = inc;
+  __syncthreads();
+  float before = 0.f, total = 0.f;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) {
+    if (w < (tid >> 5)) before += sh_scan[w];
+    total += sh_scan[w];
+  }
+  const float hi = before + inc, lo = hi - mass_t;
+  const float target = u * total;
+  int pick = -1;
+  if ((target >= lo && target < hi && mass_t > 0.f) || (tid == 255 && target >= hi)) {
+    float acc = lo;
+    pick = i1 - 1;
+    for (int i = i0; i < i1; ++i) {
+      acc += mass(i);
+      if (target < acc) { pick = i; break; }
+    }
+  }
+  *total_out = total;
+  return block_reduce_max_int(pick, sh_pick);
+}
+
 __global__ void __launch_bounds__(256) constrained_select_kernel(const SelectParams p, const ConstrainParams q) {
   griddep_launch_early();
   StepState* st = p.state;
@@ -120,39 +173,9 @@ __global__ void __launch_bounds__(256) constrained_select_kernel(const SelectPar
   float lp = -logf(sum1);                   // z[arg] - max - log(sum exp(z - max)) with z[arg] == max
   int next_node = -1;
   if (sampling && !rs.done && !rs.in_prefix) {
-    // inclusive scan of the 256 thread masses in thread order (warp scans + the 8 warp totals in order)
-    float inc = sT;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const float up = __shfl_up_sync(0xffffffffu, inc, o);
-      if ((tid & 31) >= o) inc += up;
-    }
-    if ((tid & 31) == 31) sh_scan[tid >> 5] = inc;
-    __syncthreads();
-    float before = 0.f, total = 0.f;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) {
-      if (w < (tid >> 5)) before += sh_scan[w];
-      total += sh_scan[w];
-    }
-    const float hi = before + inc, lo = hi - sT;
     const float u = __ldg(q.uniforms + static_cast<long long>(cur_len) * p.rows_total + p.row0 + row);
-    const float target = u * total;
-    if (tid == 0) { sh_i[0] = -1; }
-    __syncthreads();
-    // the owner of the interval [lo, hi) that holds the target walks its indices; a target at or beyond the total (u -> 1
-    // and rounding) falls to the last thread, whose walk ends at the last index
-    if ((target >= lo && target < hi && sT > 0.f) || (tid == 255 && target >= hi)) {
-      float acc = lo;
-      int pick = i1 - 1;
-      for (int i = i0; i < i1; ++i) {
-        acc += __expf((val(i) - gmax) * it);
-        if (target < acc) { pick = i; break; }
-      }
-      atomicMax(&sh_i[0], pick);            // at most two threads can qualify (interval owner + the last thread)
-    }
-    __syncthreads();
-    int pick = sh_i[0];
+    float total;
+    int pick = inverse_cdf_index(sT, u, i0, i1, [&](int i) { return __expf((val(i) - gmax) * it); }, sh_scan, sh_arg, &total);
     if (pick < 0) pick = garg;
     tok = pick;
     const float vz = val(pick);

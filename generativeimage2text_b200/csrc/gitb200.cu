@@ -45,7 +45,7 @@
 using namespace gitb200;
 typedef __nv_bfloat16 bf16;
 
-#define GITB200_ABI_VERSION 10
+#define GITB200_ABI_VERSION 11
 
 // ------------------------------------------------------------------------------------------------
 // errors
@@ -206,6 +206,7 @@ struct gitb200_engine {
   StepState* host_state = nullptr;   // pinned
   bool pending = false;
   int pend_max_steps = 0;
+  int pend_rows = 0;                               // rows of the call in flight (beam: B * beam)
   bool pend_beam = false;
   cudaStream_t pend_stream = nullptr;
   cudaEvent_t chunk_ev[2] = {nullptr, nullptr};   // decode-loop chunks (generate_impl)
@@ -224,6 +225,10 @@ struct gitb200_engine {
     const float* uniforms = nullptr;      // sampling (gitb200_set_sampling)
     int sample_steps = 0, sample_rows = 0;
     float temperature = 1.0f;
+    const float* beam_uniforms = nullptr; // sampled beam search (gitb200_set_beam_sampling)
+    int beam_sample_steps = 0, beam_sample_rows = 0;
+    float beam_temperature = 1.0f, beam_top_p = 1.0f;
+    int beam_top_k = 0;
   } next;
 };
 
@@ -767,7 +772,7 @@ __global__ void sum_partials_kernel(const float* __restrict__ parts, float* __re
 }
 __global__ void set_state_kernel(StepState* st, int pos, int cur_len, unsigned int* chain) {
   st->pos = pos; st->cur_len = cur_len; st->finished = 0; st->final_len = cur_len; st->step = 0;
-  st->empty_caption = 0; st->ticket = 0; st->not_eos = 0; st->error = 0;
+  st->empty_caption = 0; st->ticket = 0; st->not_eos = 0; st->error = 0; st->bad_draw = 0;
   for (int k = 0; k < 64; ++k) chain[k] = 0;
 }
 __global__ void init_generate_kernel(long long* tokens_out, long long* next_token, float* logprob_sum,

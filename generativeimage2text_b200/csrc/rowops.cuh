@@ -18,6 +18,8 @@ struct StepState {
   unsigned int ticket;
   int not_eos;        // rows whose newest token is not EOS (per step, reset by the last block)
   int error;          // decode_mega_kernel: the MegaWaitError of the first bounded wait that gave up (0: none)
+  int bad_draw;       // beam_sample_kernel: 0x7fffffff - (step * rows + row) of the first row with fewer than two tokens
+                      // to draw from (0: none)
 };
 
 // Why a bounded wait of decode_mega_kernel gave up: a protocol bug ends in one of these codes, not in a hung device.

@@ -18,6 +18,7 @@
 // different logits of one row to the same score (e.g. z - max = -100 for a logit one ulp apart), and those keep the logit
 // order -- the order of their exact scores.  The merge breaks equal scores of different beams by the lower flat index.
 #pragma once
+#include "constrained.cuh"
 #include "ptx.cuh"
 #include "rowops.cuh"
 
@@ -54,8 +55,19 @@ struct BeamState {
   long long* hyp_tok;     // [B, max_steps]
 };
 
+// The do_sample branch of GeneratorWithBeamSearch.search (reference layers/decoder.py:1138-1166): uniforms == null is the
+// deterministic search.
+struct BeamSample {
+  const float* uniforms;  // [max_steps, rows, 2]: row r at caption length t draws with uniforms[(t * rows + r) * 2 + d]
+  float temperature;
+  int top_k;              // <= 0: no top-k filter
+  float top_p;            // 0 or >= 1: no nucleus filter
+  int* kept;              // optional [rows]: size of each row's kept set (test hook)
+};
+
 struct BeamParams {
   BeamState s;
+  BeamSample smp;
   const float* logits;    // [rows, V]
   int V, B, beam, per_node, max_steps, T_alloc, eos;
   float length_penalty;
@@ -171,6 +183,282 @@ __global__ void __launch_bounds__(256) beam_row_topk_kernel(const BeamParams p) 
   }
 }
 
+// ---- sampled beam search ---------------------------------------------------------------------------------------------
+// beam_sample_kernel replaces beam_row_topk_kernel when BeamParams::smp.uniforms is set.  Per row (reference
+// layers/decoder.py:1140-1161, top_k_top_p_filtering :1343-1375): scores = logits / T; top-k keeps the values >= the k-th
+// largest (k = min(max(top_k, 2), V); ties at it all kept); top-p sorts by (value desc, index asc -- torch.sort leaves ties
+// unordered, this is the engine's order), finds the first position J whose cumulative softmax exceeds p and keeps the
+// positions 0 .. max(J, 2) (the first two are forced, then the mask shifts right by one); two draws without replacement
+// from softmax(kept), each an index-order inverse-CDF lookup with its own uniform; candidate d of the row =
+// log_softmax(kept)[token_d] + beam_score[row].  No sort: the k-th value and the top-p boundary come from radix descents
+// over the order-preserving keys of the scores.  Every sum runs in a fixed order, so results are bit-reproducible.
+constexpr int kSampleMaxVocab = 48 * 1024;   // the row's scores are kept in shared memory
+
+__device__ __forceinline__ unsigned int order_key(float v) {   // uint32 order == fp32 order
+  const unsigned int b = __float_as_uint(v);
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ float key_value(unsigned int k) {
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
+__device__ __forceinline__ int block_exclusive_scan_int(int v, int* sh) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int inc = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int up = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += up;
+  }
+  if (lane == 31) sh[warp] = inc;
+  __syncthreads();
+  int before = 0;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) if (w < warp) before += sh[w];
+  __syncthreads();
+  return before + inc - v;
+}
+
+struct SampleSmem {
+  int cnt[8][256];      // per-warp digit histograms: counts ...
+  float mass[8][256];   // ... and masses
+  float stage[8][32];
+  int scan_c[256];      // inclusive scans over the buckets, in descending key order
+  float scan_m[256];
+  float red[8];
+  int ired[8];
+};
+
+// Where a descending walk over the keys stops: the key, how many keys lie strictly above it (and their mass), how many
+// equal it.  found = false: the mass never exceeds the target.
+struct RadixStop {
+  unsigned int key;
+  int above, equal;
+  float mass_above;
+  bool found;
+};
+
+// MSB-first radix descent over the keys of s[0 .. V), 8 bits per pass, buckets visited in descending key order.
+//   kMass = false: stops at the key of the `want`-th largest value (1-based, duplicates counted).
+//   kMass = true : stops at the key where the running mass first exceeds `want`; the mass of s_i is exp(s_i - m), over
+//                  the keys >= live only (`above` / `equal` count those).
+// The histograms are per warp and need no atomics: the lanes of a warp that share a digit add their count (and their
+// masses, lane by lane) through the lowest of them.  Bucket totals add the warps in order and the bucket scan is a fixed
+// shuffle tree, so the masses are summed in one fixed order.  When rounding leaves a later pass without a crossing (its
+// buckets need not add up to the total the pass before saw), the descent takes the lowest non-empty bucket.
+template <bool kMass>
+__device__ RadixStop radix_descend(const float* s, int V, float want, unsigned int live, float m, SampleSmem& sm) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  RadixStop r{0u, 0, 0, 0.f, true};
+  unsigned int mask = 0u;
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    for (int d = lane; d < 256; d += 32) {
+      sm.cnt[warp][d] = 0;
+      if (kMass) sm.mass[warp][d] = 0.f;
+    }
+    __syncwarp();
+    for (int base = 0; base < V; base += 256) {
+      const int i = base + tid;
+      unsigned int key = 0u;
+      bool in = false;
+      if (i < V) {
+        key = order_key(s[i]);
+        in = (key & mask) == r.key && (!kMass || key >= live);   // mass: only the top-k survivors can hold the crossing
+      }
+      if (!__any_sync(0xffffffffu, in)) continue;
+      const unsigned int digit = (key >> shift) & 255u;
+      const unsigned int grp = __match_any_sync(0xffffffffu, in ? digit : 0x100u);
+      if (kMass) {
+        sm.stage[warp][lane] = in ? expf(s[i] - m) : 0.f;
+        __syncwarp();
+      }
+      if (in && lane == __ffs(grp) - 1) {
+        sm.cnt[warp][digit] += __popc(grp);
+        if (kMass) {
+          float acc = 0.f;
+          for (unsigned int g = grp; g != 0u; g &= g - 1u) acc += sm.stage[warp][__ffs(g) - 1];
+          sm.mass[warp][digit] += acc;
+        }
+      }
+      __syncwarp();
+    }
+    __syncthreads();
+    const int d = 255 - tid;   // thread t: bucket 255 - t
+    int c = 0;
+    float ms = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) {
+      c += sm.cnt[w][d];
+      if (kMass) ms += sm.mass[w][d];
+    }
+    int ci = c;
+    float mi = ms;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int cu = __shfl_up_sync(0xffffffffu, ci, o);
+      const float mu = __shfl_up_sync(0xffffffffu, mi, o);
+      if (lane >= o) { ci += cu; mi += mu; }
+    }
+    if (lane == 31) { sm.ired[warp] = ci; sm.red[warp] = mi; }
+    __syncthreads();
+#pragma unroll
+    for (int w = 0; w < 8; ++w) {
+      if (w < warp) { ci += sm.ired[w]; if (kMass) mi += sm.red[w]; }
+    }
+    __syncthreads();
+    sm.scan_c[tid] = ci;
+    if (kMass) sm.scan_m[tid] = mi;
+    const bool stop = kMass ? (c > 0 && r.mass_above + mi > want) : (static_cast<float>(r.above + ci) >= want);
+    int t = 255 - block_reduce_max_int(stop ? 255 - tid : -1, sm.ired);   // the first bucket that stops (256: none)
+    if (t > 255) {
+      if (kMass && shift == 24) { r.found = false; return r; }
+      t = block_reduce_max_int(c > 0 ? tid : -1, sm.ired);
+    }
+    const int c_before = t > 0 ? sm.scan_c[t - 1] : 0;
+    r.above += c_before;
+    if (kMass && t > 0) r.mass_above += sm.scan_m[t - 1];
+    r.equal = sm.scan_c[t] - c_before;
+    r.key |= static_cast<unsigned int>(255 - t) << shift;
+    mask |= 255u << shift;
+    __syncthreads();
+  }
+  return r;
+}
+
+__global__ void __launch_bounds__(256) beam_sample_kernel(const BeamParams p) {
+  griddep_launch();
+  griddep_wait();
+  StepState* st = p.state;
+  if (st->finished) return;
+  extern __shared__ float srow[];   // the row's scores logits / T
+  __shared__ SampleSmem sm;
+  const int row = blockIdx.x, rows = gridDim.x, tid = threadIdx.x, V = p.V;
+  const int cur_len = st->cur_len;
+  const float* z = p.logits + static_cast<long long>(row) * V;
+  float* dump = p.step_logits != nullptr ? p.step_logits + (static_cast<long long>(st->step) * rows + row) * V : nullptr;
+  float mx = -INFINITY;
+  for (int i0 = tid; i0 < V; i0 += 8 * 256) {        // 8 independent loads in flight per thread
+    float v[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) v[k] = (i0 + k * 256 < V) ? __ldcg(z + i0 + k * 256) : 0.f;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const int i = i0 + k * 256;
+      if (i >= V) break;
+      if (dump != nullptr) dump[i] = v[k];
+      const float sv = v[k] / p.smp.temperature;   // a division, as the reference: a multiply by 1/T can split a tie it makes
+      srow[i] = sv;
+      mx = fmaxf(mx, sv);
+    }
+  }
+  // an image still inside its prefix takes the prefix token (beam_update_kernel): nothing to draw
+  if (p.row_prefix != nullptr && cur_len < p.row_prefix_lens[row / p.beam]) return;
+  const float m = block_reduce_max(mx, sm.red);
+
+  // ---- top-k: keys >= live survive ----
+  unsigned int live = 0u;
+  int n_live = V;
+  if (p.smp.top_k > 0) {
+    const RadixStop r = radix_descend<false>(srow, V, static_cast<float>(min(max(p.smp.top_k, 2), V)), 0u, m, sm);
+    live = r.key;
+    n_live = r.above + r.equal;
+  }
+  // ---- top-p: kept = keys > kkey, and the keys == kkey up to index i_last ----
+  unsigned int kkey = live;
+  int keep_ties = 0x7fffffff, n_kept = n_live;
+  const float top_p = p.smp.top_p;
+  if (top_p != 0.f && top_p < 1.f) {
+    float w = 0.f;
+    for (int i = tid; i < V; i += 256)
+      if (order_key(srow[i]) >= live) w += expf(srow[i] - m);
+    const float target = top_p * block_reduce_sum(w, sm.red);   // cumsum(softmax) > p  <=>  cumsum(exp(s - m)) > p * sum
+    const RadixStop c = radix_descend<true>(srow, V, target, live, m, sm);
+    if (c.found) {
+      // the position J where the cumulative mass crosses: the first j of the c.equal ties at c.key (index order), each of
+      // mass q, with mass_above + (j + 1) q > target (computed, not accumulated: thousands of equal terms would drift)
+      const float q = expf(key_value(c.key) - m);
+      const float n = floorf((target - c.mass_above) / q);
+      const int j = !(n > 0.f) ? 0 : (n >= static_cast<float>(c.equal - 1) ? c.equal - 1 : static_cast<int>(n));
+      const int J = c.above + j;
+      const int K = max(J, 2) + 1;   // positions 0 .. max(J, 2): the first two forced, then the shift right by one
+      if (K < n_live) {
+        n_kept = K;
+        if (J >= 2) {
+          kkey = c.key;
+          keep_ties = j + 1;
+        } else {
+          const RadixStop r3 = radix_descend<false>(srow, V, 3.f, 0u, m, sm);
+          kkey = r3.key;
+          keep_ties = 3 - r3.above;
+        }
+      }
+    }
+  }
+  // thread t owns the contiguous indices [i0, i1): ties and draws go in index order (an odd stride: no bank conflicts)
+  const int C = ((V + 255) / 256) | 1;
+  const int i0 = min(V, tid * C), i1 = min(V, i0 + C);
+  int i_last = V;
+  if (keep_ties != 0x7fffffff) {
+    int nt = 0;
+    for (int i = i0; i < i1; ++i) nt += order_key(srow[i]) == kkey;
+    const int before = block_exclusive_scan_int(nt, sm.ired);
+    int found = -1;
+    if (keep_ties > before && keep_ties <= before + nt) {
+      int k = before;
+      for (int i = i0; i < i1; ++i)
+        if (order_key(srow[i]) == kkey && ++k == keep_ties) { found = i; break; }
+    }
+    i_last = block_reduce_max_int(found, sm.ired);
+  }
+  auto mass = [&](int i) -> float {
+    const unsigned int k = order_key(srow[i]);
+    return (k > kkey || (k == kkey && i <= i_last)) ? expf(srow[i] - m) : 0.f;
+  };
+
+  // ---- two draws without replacement ----
+  float w1 = 0.f;
+  int nz1 = -1;
+  for (int i = i0; i < i1; ++i) {
+    const float w = mass(i);
+    w1 += w;
+    if (w > 0.f) nz1 = i;
+  }
+  const int last1 = block_reduce_max_int(nz1, sm.ired);
+  const float* u = p.smp.uniforms + (static_cast<long long>(cur_len) * rows + row) * 2;
+  float total1 = 0.f, total2 = 0.f;
+  int t1 = inverse_cdf_index(w1, __ldg(u), i0, i1, mass, sm.red, sm.ired, &total1);
+  if (t1 < 0 || !(mass(t1) > 0.f)) t1 = last1;   // rounding at the end of the distribution: never a zero-probability token
+  auto mass2 = [&](int i) -> float { return i == t1 ? 0.f : mass(i); };
+  float w2 = w1;
+  int nz2 = nz1;
+  if (t1 >= i0 && t1 < i1) {
+    w2 = 0.f;
+    nz2 = -1;
+    for (int i = i0; i < i1; ++i) {
+      const float w = mass2(i);
+      w2 += w;
+      if (w > 0.f) nz2 = i;
+    }
+  }
+  const int last2 = block_reduce_max_int(nz2, sm.ired);
+  int t2 = inverse_cdf_index(w2, __ldg(u + 1), i0, i1, mass2, sm.red, sm.ired, &total2);
+  if (t2 < 0 || !(mass2(t2) > 0.f)) t2 = last2;
+  if (tid != 0) return;
+  if (!(m > -INFINITY) || !(total2 > 0.f)) {
+    // torch.multinomial raises: fewer than two tokens of non-zero probability.  The first such (step, row) is reported
+    // by gitb200_generate_finish; the search stops.
+    atomicMax(&st->bad_draw, 0x7fffffff - (st->step * rows + row));
+    st->finished = 1;
+    return;
+  }
+  const float lse = logf(total1), bs = p.s.beam_scores[row];
+  p.s.cand_val[row * kMaxCand] = ((srow[t1] - m) - lse) + bs;
+  p.s.cand_idx[row * kMaxCand] = t1;
+  p.s.cand_val[row * kMaxCand + 1] = ((srow[t2] - m) - lse) + bs;
+  p.s.cand_idx[row * kMaxCand + 1] = t2;
+  if (p.smp.kept != nullptr) p.smp.kept[row] = n_kept;
+}
+
 // One thread block per image (32 threads; the bookkeeping itself is sequential like the reference's loop).
 __global__ void __launch_bounds__(32) beam_update_kernel(const BeamParams p) {
   griddep_launch();
@@ -202,29 +490,45 @@ __global__ void __launch_bounds__(32) beam_update_kernel(const BeamParams p) {
     }
   }
   if (lane == 0 && !in_prefix) {
-    // merge the `beam` row lists into the image's top-NC, ordered by (value desc, flat index asc)
-    int ptr[kMaxBeam];
-    for (int k = 0; k < beam; ++k) ptr[k] = 0;
-    for (int c = 0; c < NC; ++c) {
-      int best = -1;
-      float bv = 0.f;
-      long long bflat = 0;
-      for (int k = 0; k < beam; ++k) {
-        if (ptr[k] >= NC) continue;
-        const int r = b * beam + k;
-        const float v = p.s.cand_val[r * kMaxCand + ptr[k]];
-        const long long flat = static_cast<long long>(k) * V + p.s.cand_idx[r * kMaxCand + ptr[k]];
-        if (best < 0 || v > bv || (v == bv && flat < bflat)) { best = k; bv = v; bflat = flat; }
+    float top;   // the best candidate score
+    if (p.smp.uniforms != nullptr) {
+      // sampled candidates stay in (beam, draw) order (reference :1159-1166); is_done takes their maximum (:1187).  The
+      // reference offsets candidate c by the beam index tiled as [0 .. beam) x per_node (:1155-1158), so the history that
+      // candidate c (row c / per_node's draw c % per_node) extends is that of beam c % beam.
+      top = -INFINITY;
+      for (int c = 0; c < NC; ++c) {
+        const int r = b * beam + c / p.per_node;
+        m_val[c] = p.s.cand_val[r * kMaxCand + c % p.per_node];
+        m_word[c] = p.s.cand_idx[r * kMaxCand + c % p.per_node];
+        m_beam[c] = c % beam;
+        top = fmaxf(top, m_val[c]);
       }
-      m_val[c] = bv;
-      m_word[c] = p.s.cand_idx[(b * beam + best) * kMaxCand + ptr[best]];
-      m_beam[c] = best;
-      ++ptr[best];
+    } else {
+      // merge the `beam` row lists into the image's top-NC, ordered by (value desc, flat index asc)
+      int ptr[kMaxBeam];
+      for (int k = 0; k < beam; ++k) ptr[k] = 0;
+      for (int c = 0; c < NC; ++c) {
+        int best = -1;
+        float bv = 0.f;
+        long long bflat = 0;
+        for (int k = 0; k < beam; ++k) {
+          if (ptr[k] >= NC) continue;
+          const int r = b * beam + k;
+          const float v = p.s.cand_val[r * kMaxCand + ptr[k]];
+          const long long flat = static_cast<long long>(k) * V + p.s.cand_idx[r * kMaxCand + ptr[k]];
+          if (best < 0 || v > bv || (v == bv && flat < bflat)) { best = k; bv = v; bflat = flat; }
+        }
+        m_val[c] = bv;
+        m_word[c] = p.s.cand_idx[(b * beam + best) * kMaxCand + ptr[best]];
+        m_beam[c] = best;
+        ++ptr[best];
+      }
+      top = m_val[0];
     }
     // ---- reference bookkeeping (layers/decoder.py:1184-1228) ----
     bool done = p.s.done[b] != 0;
     if (!done && p.s.hyp_len[b] > 0) {  // BeamHypotheses.is_done with early_stopping=False (:1330-1341)
-      done = p.s.worst_score[b] >= m_val[0] / beam_length_norm(p.max_steps - 1, p.length_penalty);
+      done = p.s.worst_score[b] >= top / beam_length_norm(p.max_steps - 1, p.length_penalty);
     }
     p.s.done[b] = done ? 1 : 0;
     int n_next = 0;

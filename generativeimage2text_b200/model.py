@@ -39,7 +39,9 @@ class AutoRegressiveBeamSearch(object):
 
 class GeneratorWithBeamSearch(object):
     """Search configuration mirroring reference layers/decoder.py:1056-1081 (the shipped default:
-    beam 4, per-node 2, length_penalty 0.6, model.py:34-40)."""
+    beam 4, per-node 2, length_penalty 0.6, model.py:34-40).  The constructor takes temperature 1 only; sampled beam search
+    (search_param={'do_sample': True, ...}) divides the logits by the `temperature` attribute, the value the reference's
+    search reads (layers/decoder.py:1097, 1140-1142), so `decoder.temperature = 0.7` sets it."""
 
     def __init__(self, eos_index, max_steps, beam_size, per_node_beam_size=2, length_penalty=1,
                  repetition_penalty=1, temperature=1):
@@ -54,8 +56,27 @@ class GeneratorWithBeamSearch(object):
         assert self.length_penalty > 0, "`length_penalty` should be strictely positive."
         assert self.repetition_penalty >= 1.0, "`repetition_penalty` should be >= 1."
         assert self.temperature > 0, "`temperature` should be strictely positive."
-        if repetition_penalty != 1 or temperature != 1:
-            raise NotImplementedError('repetition_penalty / temperature are not used by get_git_model')
+        if repetition_penalty != 1:
+            raise NotImplementedError('repetition_penalty is not implemented')
+        if temperature != 1:
+            raise NotImplementedError('temperature is not a constructor argument here: sampled beam search reads the '
+                                      'decoder\'s `temperature` attribute (decoder.temperature = T)')
+
+
+class BeamSampleArgumentError(TypeError, NotImplementedError):
+    """Sampled beam search called without an integer top_k.  The reference raises TypeError there (`top_k > 0` with its
+    default None, layers/decoder.py:1355); a sampling call this package cannot run raises NotImplementedError.  The error
+    is both, so callers written against either keep working."""
+
+
+def _beam_filter(search_param):
+    """(top_k, top_p) of a sampled GeneratorWithBeamSearch call as the engine takes them.  The reference tests `top_k > 0`
+    (layers/decoder.py:1355) and `top_p and top_p < 1.0` (:1359): top_k must be an integer (0: no top-k filter), a false
+    top_p means no nucleus filter."""
+    top_k, top_p = search_param.get('top_k'), search_param.get('top_p')
+    if isinstance(top_k, bool) or not isinstance(top_k, int):
+        raise BeamSampleArgumentError('sampled beam search needs an integer top_k (0: no top-k filter), got %r' % (top_k,))
+    return top_k, (float(top_p) if top_p else 1.0)
 
 
 class TokenNode(object):
@@ -487,7 +508,10 @@ class GitB200CaptioningModel(nn.Module):
         search_param: the dict CaptioningModel.infer forwards to decoder.search (layers/decoder.py:999-1003); understood:
                {'do_sample': True, 'temperature': T, 'top_k': ., 'top_p': .} with the greedy decoder -- top_k / top_p are
                accepted and ignored exactly like the reference (its filter call is commented out, :372) -- plus
-               'uniforms': FloatTensor[max_steps, B] or 'generator': torch.Generator for the random numbers.
+               'uniforms': FloatTensor[max_steps, B] or 'generator': torch.Generator for the random numbers;
+               {'do_sample': True, 'top_k': int, 'top_p': .} with GeneratorWithBeamSearch (the temperature is the
+               decoder's `temperature` attribute; num_keep_best / num_return_sequences only 1) plus 'uniforms': FloatTensor[max_steps,
+               B * beam_size, 2] or 'generator'.
         """
         return self.submit(batch, forced_tokens, return_step_logits, slot=0, _caller_stream=True,
                            search_param=search_param).result()
@@ -582,7 +606,11 @@ class GitB200CaptioningModel(nn.Module):
             _lib.check(lib.gitb200_set_row_prefixes(eng, row_prefix.data_ptr(), B, int(row_prefix.shape[1]), row_lens_dev.data_ptr()),
                        eng, 'set_row_prefixes')
         self._trie_setup(lib, sl)
-        if uniforms is not None:
+        if uniforms is not None and sp.mode == _lib.SEARCH_BEAM:
+            top_k, top_p = _beam_filter(search_param)
+            _lib.check(lib.gitb200_set_beam_sampling(eng, uniforms.data_ptr(), int(uniforms.shape[0]), int(uniforms.shape[1]),
+                                                     float(self.decoder.temperature), top_k, top_p), eng, 'set_beam_sampling')
+        elif uniforms is not None:
             _lib.check(lib.gitb200_set_sampling(eng, uniforms.data_ptr(), int(uniforms.shape[0]), B,
                                                 float(search_param.get('temperature', 1))), eng, 'set_sampling')
         _lib.check(lib.gitb200_generate_async(
@@ -667,15 +695,19 @@ class GitB200CaptioningModel(nn.Module):
         return {'token_logprobs': lp, 'vl_l_loss': loss[0]}
 
     def _sampling_setup(self, search_param, sp, B, dev):
-        """search_param of the reference's decoder.search (layers/decoder.py:224-232) -> the uniforms the engine draws with."""
+        """search_param of the reference's decoder.search (layers/decoder.py:224-232, 1083-1092) -> the uniforms the engine
+        draws with (None: a deterministic search)."""
         if not search_param:
             return None
+        if isinstance(self.decoder, GeneratorWithBeamSearch):
+            return self._beam_sampling_setup(search_param, sp, B, dev)
         unknown = set(search_param) - {'do_sample', 'temperature', 'top_k', 'top_p', 'num_return_sequences', 'uniforms',
                                        'generator', 'only_return_best'}
         if unknown:
             raise TypeError('unknown search_param keys: %s' % sorted(unknown))
         if not isinstance(self.decoder, AutoRegressiveBeamSearch):
-            raise NotImplementedError('search_param (sampling) is implemented for AutoRegressiveBeamSearch only')
+            raise NotImplementedError('search_param (sampling) is implemented for AutoRegressiveBeamSearch and '
+                                      'GeneratorWithBeamSearch only')
         if search_param.get('num_return_sequences', 1) != 1 or not search_param.get('only_return_best', True):
             raise NotImplementedError('num_return_sequences > 1 / only_return_best=False are not implemented')
         temperature = float(search_param.get('temperature', 1))
@@ -690,6 +722,35 @@ class GitB200CaptioningModel(nn.Module):
         u = u.to(device=dev, dtype=torch.float32).contiguous()
         if u.dim() != 2 or u.shape[0] < sp.max_steps or u.shape[1] != B:
             raise ValueError("'uniforms' must be a [>= max_steps, B] tensor")
+        return u
+
+    def _beam_sampling_setup(self, search_param, sp, B, dev):
+        """GeneratorWithBeamSearch.search(input_ids, step, num_keep_best, do_sample, top_k, top_p, num_return_sequences)
+        (reference layers/decoder.py:1083-1092); its temperature is the decoder's `temperature` attribute (:1097).  -> uniforms
+        [max_steps, B * beam_size, 2], or None when do_sample is off (top_k / top_p are then unused, as in the reference)."""
+        if 'temperature' in search_param:
+            raise TypeError("GeneratorWithBeamSearch.search() got an unexpected keyword argument 'temperature' (sampled "
+                            "beam search divides by the decoder's `temperature` attribute)")
+        unknown = set(search_param) - {'do_sample', 'top_k', 'top_p', 'uniforms', 'generator', 'num_keep_best',
+                                       'num_return_sequences'}
+        if unknown:
+            raise NotImplementedError('search_param keys not implemented for GeneratorWithBeamSearch: %s' % sorted(unknown))
+        for key in ('num_keep_best', 'num_return_sequences'):
+            if search_param.get(key, 1) != 1:
+                raise NotImplementedError('%s > 1 is not implemented' % key)
+        if not search_param.get('do_sample', False):
+            return None
+        _beam_filter(search_param)
+        temperature = self.decoder.temperature
+        if not (isinstance(temperature, (int, float)) and 0 < temperature < float('inf')):
+            raise ValueError('decoder.temperature must be a positive number (got %r)' % (temperature,))
+        rows = B * sp.beam_size
+        u = search_param.get('uniforms')
+        if u is None:
+            u = torch.rand((sp.max_steps, rows, 2), dtype=torch.float32, device=dev, generator=search_param.get('generator'))
+        u = u.to(device=dev, dtype=torch.float32).contiguous()
+        if u.dim() != 3 or u.shape[0] < sp.max_steps or u.shape[1] != rows or u.shape[2] != 2:
+            raise ValueError("'uniforms' must be a [>= max_steps, B * beam_size, 2] tensor")
         return u
 
     def _trie_setup(self, lib, sl):
@@ -725,8 +786,9 @@ class GitB200CaptioningModel(nn.Module):
         lib = _lib.load()
         sl = self._slots[pend.slot]
         out_len = ctypes.c_int32(0)
-        _lib.check(lib.gitb200_generate_finish(sl['engine'], ctypes.byref(out_len)), sl['engine'], 'generate_finish')
-        sl['pending'] = None
+        rc = lib.gitb200_generate_finish(sl['engine'], ctypes.byref(out_len))
+        sl['pending'] = None                  # finished either way: the engine takes the next call
+        _lib.check(rc, sl['engine'], 'generate_finish')
         sp, P, tokens, logprobs = pend.sp, pend.P, pend.tokens, pend.logprobs
         n = out_len.value
         if pend.row_lens is not None:

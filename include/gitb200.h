@@ -62,8 +62,8 @@ enum { GITB200_F32 = 0, GITB200_BF16 = 1, GITB200_I64 = 2 };
 int gitb200_create(const gitb200_config* cfg, int device, gitb200_engine** out);
 void gitb200_destroy(gitb200_engine* h);
 const char* gitb200_last_error(const gitb200_engine* h);
-/* ABI version of the library (bumped on any signature change): 10 (gitb200_op_gemm_ex, gitb200_op_layernorm_ex,
- * gitb200_op_lse_combine); 9 added gitb200_score and gitb200_op_text_attention. */
+/* ABI version of the library (bumped on any signature change): 11 (gitb200_set_beam_sampling, gitb200_op_beam_sample);
+ * 10 added gitb200_op_gemm_ex, gitb200_op_layernorm_ex and gitb200_op_lse_combine; 9 added gitb200_score and gitb200_op_text_attention. */
 int gitb200_abi_version(void);
 
 /* Replaces: torch_common.load_state_dict -> module parameters           torch_common.py:93-145.
@@ -105,9 +105,9 @@ int gitb200_set_input_size(gitb200_engine* h, int height, int width);
  * and frames must be 0 or 1.  Image b has L_b = (H_b / patch) * (W_b / patch) + 1 tokens in a slot of L_max = max L_b
  * rows: row b of the results is what a batch-1 call with that image alone returns.  The greedy decode steps of such a
  * call run on the kernel chain (use_mega does not apply).  gitb200_set_input_size is left as it was.
- * Inputs of the next call only (this one, gitb200_set_row_prefixes, gitb200_set_sampling): the next call that can use
- * them takes them at entry, right after its in-flight check -- gitb200_encode and gitb200_score take the image sizes, a
- * gitb200_generate* call takes all three -- and they are gone from the engine whether that call succeeds or fails. */
+ * Inputs of the next call only (this one, gitb200_set_row_prefixes, gitb200_set_sampling, gitb200_set_beam_sampling): the
+ * next call that can use them takes them at entry, right after its in-flight check -- gitb200_encode and gitb200_score take
+ * the image sizes, a gitb200_generate* call takes all four -- and they are gone from the engine whether that call succeeds or fails. */
 int gitb200_set_image_sizes(gitb200_engine* h, const int32_t* hw_host, int n);
 
 /* Replaces: visual_projection + the image rows of BertEncoderAsDecoder, computed once (KV cache)
@@ -199,6 +199,19 @@ int gitb200_set_trie(gitb200_engine* h, const int32_t* child_begin_host, const i
  * be reproduced, the distribution is the same).  Log-probs as the reference computes them: tempered log-softmax at a
  * row's first decision, un-tempered afterwards.  The buffer must stay valid until the call has finished. */
 int gitb200_set_sampling(gitb200_engine* h, const float* uniforms_dev, int steps, int rows, float temperature);
+
+/* Replaces: the do_sample branch of GeneratorWithBeamSearch.search                layers/decoder.py:1138-1166, 1343-1375
+ * for the NEXT generate call, which must be a beam search (per_node_beam 2) and takes them as gitb200_set_image_sizes
+ * describes.  Every step, row r (of rows == batch * beam_size) filters scores = logits / temperature by top_k (<= 0: off;
+ * k = min(max(top_k, 2), V), ties at the k-th value kept) and top_p (0 or >= 1: off; sorted by value desc, index asc, the
+ * positions up to the first whose cumulative softmax exceeds top_p are kept, and never fewer than three), then draws two
+ * tokens without replacement from softmax(filtered), each by an inverse-CDF lookup in index order with
+ * uniforms_dev[(t * rows + r) * 2 + d] at caption length t (fp32 [steps >= max_steps, rows, 2], device).  A candidate's
+ * score is log_softmax(filtered)[token] + the row's beam score; the candidates of an image stay in (beam, draw) order.
+ * A row with fewer than two tokens of non-zero probability stops the search, and gitb200_generate_finish (or the
+ * synchronous generate call) fails naming its step and row.  The buffer must stay valid until the call has finished. */
+int gitb200_set_beam_sampling(gitb200_engine* h, const float* uniforms_dev, int steps, int rows, float temperature,
+                              int top_k, float top_p);
 
 /* Number of kernels the engine launched since creation (bench.py's gpu_launches). */
 int64_t gitb200_launch_count(const gitb200_engine* h);
@@ -292,6 +305,15 @@ int gitb200_op_decode_attention(const float* qkv_dev, int n_partials, const floa
                                 const void* img_v_dev, void* txt_k_dev, void* txt_v_dev, const int32_t* src_row_dev,
                                 void* ctx_dev, int B, int beam, int M, const int32_t* img_lens_host, int T_alloc, int pos,
                                 int D, int fp32, int grid, void* stream);
+
+/* One step of sampled beam search's per-row selection (beam_sample_kernel, see gitb200_set_beam_sampling) on given logits:
+ * logits_dev fp32 [rows, V] (V <= 49152), beam_scores_dev fp32 [rows], uniforms_dev fp32 [rows, 2].  Writes the two
+ * candidates of each row, cand_val_out_dev fp32 [rows, 2] (log_softmax(filtered)[token] + beam score) and
+ * cand_idx_out_dev int32 [rows, 2], and kept_out_dev int32 [rows] = the size of the row's kept set.  Synchronises the
+ * stream; fails when a row has fewer than two tokens of non-zero probability. */
+int gitb200_op_beam_sample(const float* logits_dev, int rows, int V, const float* beam_scores_dev, const float* uniforms_dev,
+                           float temperature, int top_k, float top_p, float* cand_val_out_dev, int32_t* cand_idx_out_dev,
+                           int32_t* kept_out_dev, void* stream);
 
 /* Caption scoring's attention (text_attn_wgmma_kernel, or text_attn_f32_kernel when fp32 != 0): text row t of caption n
  * attends to the image keys of image image_index[n] and to text keys 0 .. t of caption n; softmax(q k^T / 8) v per head.
