@@ -439,16 +439,8 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
     issue_unit(0);
     if (n_units > 1) issue_unit(1);
   }
-  bool finished;
-  if (p.chain.counters != nullptr) {
-    // `finished` only changes between steps (full dependency): in a finished step no kernel waits or signals
-    finished = (p.state != nullptr && p.state->finished);
-    if (!finished) chain_wait(p.chain);
-  } else {
-    griddep_wait();
-    finished = (p.state != nullptr && p.state->finished);
-  }
-  if (finished) {  // never leave with a bulk copy in flight into this CTA's shared memory
+  if (step_wait(p.state != nullptr ? &p.state->finished : nullptr, p.chain)) {
+    // never leave with a bulk copy in flight into this CTA's shared memory
     mbar_wait(&bars[0], 0);
     if (n_units > 1) mbar_wait(&bars[1], 0);
     return;
@@ -834,15 +826,7 @@ __host__ __device__ __forceinline__ int dec_attn_f32_warp_floats(int M, int T_al
 __global__ void __launch_bounds__(128) decode_attn_f32_kernel(const DecAttnF32Params p) {
   extern __shared__ __align__(16) float attn_f32_smem[];
   griddep_launch_early();
-  bool finished;
-  if (p.chain.counters != nullptr) {
-    finished = (p.state != nullptr && p.state->finished);
-    if (!finished) chain_wait(p.chain);
-  } else {
-    griddep_wait();
-    finished = (p.state != nullptr && p.state->finished);
-  }
-  if (finished) return;
+  if (step_wait(p.state != nullptr ? &p.state->finished : nullptr, p.chain)) return;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int D = p.D, H = D / 64;
   const int pos = (p.state != nullptr) ? p.state->pos : p.pos_fixed;

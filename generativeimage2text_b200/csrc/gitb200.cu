@@ -333,6 +333,20 @@ static int get_tmap(gitb200_engine* h, const void* ptr, long long rows, long lon
   return 0;
 }
 
+// Raises `kernel`'s dynamic shared-memory limit to smem bytes on the engine's device; the attribute is set once per kernel,
+// device and larger size (the parity and decode attention kernels size their shared memory per call).
+static int set_dyn_smem(gitb200_engine* h, const void* kernel, size_t smem) {
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, size_t> done;
+  std::lock_guard<std::mutex> lock(mu);
+  size_t& have = done[{kernel, h->device}];
+  if (have < smem) {
+    CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+    have = smem;
+  }
+  return 0;
+}
+
 // ------------------------------------------------------------------------------------------------
 // GEMM launcher
 // ------------------------------------------------------------------------------------------------
@@ -348,11 +362,7 @@ struct GemmCall {
 template <int BN, int EPI>
 static int launch_gemm_inst(gitb200_engine* h, const GemmCall& c, cudaStream_t st) {
   using C = GemmCfg<BN>;
-  static bool attr_set[64] = {false};
-  if (!attr_set[h->device & 63]) {
-    CK(cudaFuncSetAttribute(gemm_bf16_wgmma<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
-    attr_set[h->device & 63] = true;
-  }
+  TRY(set_dyn_smem(h, reinterpret_cast<const void*>(gemm_bf16_wgmma<BN, EPI>), C::SMEM_BYTES));
   CUtensorMap ta, tb;
   TRY(get_tmap(h, c.A, c.p.M, c.p.K, c.lda, 128, &ta));
   TRY(get_tmap(h, c.B, c.p.N, c.p.K, c.ldb, BN, &tb));
@@ -524,20 +534,6 @@ static LnParams ln_operand(const gitb200_engine* h, const float* x, const float*
   LnParams p = ln_params(x, nullptr, nullptr, g, b, eps, of32, obf16, rows);
   p.split3 = h->parity ? 1 : 0;
   return p;
-}
-
-// Raises `kernel`'s dynamic shared-memory limit to smem bytes on the engine's device; the attribute is set once per kernel,
-// device and larger size (the parity and decode attention kernels size their shared memory per call).
-static int set_dyn_smem(gitb200_engine* h, const void* kernel, size_t smem) {
-  static std::mutex mu;
-  static std::map<std::pair<const void*, int>, size_t> done;
-  std::lock_guard<std::mutex> lock(mu);
-  size_t& have = done[{kernel, h->device}];
-  if (have < smem) {
-    CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    have = smem;
-  }
-  return 0;
 }
 
 // Self attention (attention.cuh): non-causal, B batches of S rows.  q / k / v rows q_rs / kv_rs elements apart and batches
@@ -772,7 +768,7 @@ __global__ void sum_partials_kernel(const float* __restrict__ parts, float* __re
 }
 __global__ void set_state_kernel(StepState* st, int pos, int cur_len, unsigned int* chain) {
   st->pos = pos; st->cur_len = cur_len; st->finished = 0; st->final_len = cur_len; st->step = 0;
-  st->empty_caption = 0; st->ticket = 0; st->not_eos = 0; st->error = 0; st->bad_draw = 0;
+  st->empty_caption = 0; st->ticket = 0; st->live = 0; st->error = 0; st->bad_draw = 0;
   for (int k = 0; k < 64; ++k) chain[k] = 0;
 }
 __global__ void init_generate_kernel(long long* tokens_out, long long* next_token, float* logprob_sum,

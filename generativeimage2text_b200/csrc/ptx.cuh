@@ -79,6 +79,19 @@ __device__ __forceinline__ void chain_wait(const ChainSync& c) {
     __syncthreads();
   }
 }
+// The entry of a decode-step kernel (all threads of the CTA): returns whether the step is already over, i.e. *finished is
+// non-zero (a null `finished` never is).  In a chain the flag is read before the wait: it only changes between steps
+// (full dependency), so in a finished step no kernel waits or signals.  Without a chain the kernel waits for its
+// predecessor grid, then reads the flag.
+__device__ __forceinline__ bool step_wait(const int* finished, const ChainSync& chain) {
+  if (chain.counters != nullptr) {
+    if (finished != nullptr && *finished != 0) return true;
+    chain_wait(chain);
+    return false;
+  }
+  griddep_wait();
+  return finished != nullptr && *finished != 0;
+}
 // thread 0, after a __syncthreads() that follows the CTA's last global write
 __device__ __forceinline__ void chain_signal_thread0(const ChainSync& c) {
   // release-RMW: orders this thread's (and, through the preceding bar.sync, the CTA's) prior writes before the count

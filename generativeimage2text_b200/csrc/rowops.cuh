@@ -1,5 +1,6 @@
 // Row-wise HBM-bound kernels of the GIT hot path: LayerNorm (+bias/+residual/+temporal embedding),
-// patch im2col, CLS/pos-embed/ln_pre, token embedding + LN, and the greedy selection kernels.
+// patch im2col, CLS/pos-embed/ln_pre, token embedding + LN, and the greedy selection kernels; also the CTA reductions
+// and scans, the step-logits row and the step close that every selection kernel of the decode step shares.
 // One warp per row, 128-bit loads/stores, fp32 statistics (two-pass: mean, then biased variance,
 // like torch.nn.functional.layer_norm).
 #pragma once
@@ -16,7 +17,8 @@ struct StepState {
   int step;           // number of decode steps executed so far
   int empty_caption;  // greedy step-0 special case (reference layers/decoder.py:279-291)
   unsigned int ticket;
-  int not_eos;        // rows whose newest token is not EOS (per step, reset by the last block)
+  int live;           // units still live at this step, counted by close_step and reset by the last ticket: greedy rows
+                      // whose next token is not EOS, beam-search images not yet done
   int error;          // decode_mega_kernel: the MegaWaitError of the first bounded wait that gave up (0: none)
   int bad_draw;       // beam_sample_kernel: 0x7fffffff - (step * rows + row) of the first row with fewer than two tokens
                       // to draw from (0: none)
@@ -124,14 +126,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const LnParams p) {
       bia[i] = (p.bias != nullptr) ? __ldg(reinterpret_cast<const float4*>(p.bias) + i * 32 + lane) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
   }
-  const bool chained = p.chain.counters != nullptr;
-  if (chained) {
-    if (p.skip_flag != nullptr && *p.skip_flag != 0) return;  // stable within a step
-    chain_wait(p.chain);
-  } else {
-    griddep_wait();
-    if (p.skip_flag != nullptr && *p.skip_flag != 0) return;
-  }
+  if (step_wait(p.skip_flag, p.chain)) return;
   tl_mark(2);
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= p.rows) {
@@ -513,6 +508,145 @@ __global__ void __launch_bounds__(1024) loss_mean_kernel(const float* __restrict
 }
 
 // ------------------------------------------------------------------------------------------------
+// CTA primitives of the row kernels that end a kernel-chain decode step (greedy_select_kernel below,
+// constrained_select_kernel, beam_row_topk_kernel, beam_sample_kernel): kRowThreads threads per CTA.
+// Every block reduction and scan combines the warps in warp order: bit-reproducible.
+// ------------------------------------------------------------------------------------------------
+constexpr int kRowThreads = 256;
+constexpr int kRowWarps = kRowThreads / 32;
+
+// Reduction over the CTA with `op` (every thread gets the result): a shuffle tree per warp, then the warp results folded
+// in warp order.  sh holds kRowWarps entries.
+template <class T, class Op>
+__device__ __forceinline__ T block_reduce(T v, T* sh, Op op) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = op(v, __shfl_xor_sync(0xffffffffu, v, o));
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+  __syncthreads();
+  T r = sh[0];
+#pragma unroll
+  for (int w = 1; w < kRowWarps; ++w) r = op(r, sh[w]);
+  __syncthreads();
+  return r;
+}
+__device__ __forceinline__ float block_reduce_max(float v, float* sh) {
+  return block_reduce(v, sh, [](float a, float b) { return fmaxf(a, b); });
+}
+// fixed-order sum (warp tree, then the warps in order): bit-reproducible
+__device__ __forceinline__ float block_reduce_sum(float v, float* sh) {
+  return block_reduce(v, sh, [](float a, float b) { return a + b; });
+}
+__device__ __forceinline__ int block_reduce_max_int(int v, int* sh) {
+  return block_reduce(v, sh, [](int a, int b) { return max(a, b); });
+}
+__device__ __forceinline__ int block_reduce_min_int(int v, int* sh) {
+  return block_reduce(v, sh, [](int a, int b) { return min(a, b); });
+}
+
+// Inclusive scan over the lanes of a warp: lane l gets v_0 + ... + v_l, added in the shuffle tree's order.
+template <class T>
+__device__ __forceinline__ T warp_inclusive_scan(T v) {
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const T up = __shfl_up_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) >= o) v += up;
+  }
+  return v;
+}
+
+// Exclusive prefix sum of v over the CTA's threads in thread order (sh: kRowWarps ints).
+__device__ __forceinline__ int block_exclusive_scan_int(int v, int* sh) {
+  const int warp = threadIdx.x >> 5;
+  const int inc = warp_inclusive_scan(v);
+  if ((threadIdx.x & 31) == 31) sh[warp] = inc;
+  __syncthreads();
+  int before = 0;
+#pragma unroll
+  for (int w = 0; w < kRowWarps; ++w) if (w < warp) before += sh[w];
+  __syncthreads();
+  return before + inc - v;
+}
+
+// The index-order inverse-CDF lookup of the sampling kernels (a CTA per row): thread t owns the contiguous indices
+// [i0, i1) and `mass_t` is the sum of mass(i) over them in index order.  The target is u * total, total = the thread
+// masses summed in thread order (warp scans, then the warp totals in order).  The owner of the interval [lo, hi) that
+// holds the target walks its indices to the first one whose running mass exceeds it; a target at or beyond the total
+// (u -> 1 and rounding) falls to the last thread, whose walk ends at its last index.  Rounding can make two adjacent
+// threads claim the target (lo is hi - mass_t, not the previous thread's hi): the higher index wins.  Returns the index
+// (every thread), or -1 when no thread claims the target; *total_out = total.
+template <class Mass>
+__device__ __forceinline__ int inverse_cdf_index(float mass_t, float u, int i0, int i1, Mass mass, float* sh_scan, int* sh_pick,
+                                                 float* total_out) {
+  const int tid = threadIdx.x;
+  const float inc = warp_inclusive_scan(mass_t);
+  if ((tid & 31) == 31) sh_scan[tid >> 5] = inc;
+  __syncthreads();
+  // (sum of the earlier warps' totals) + inc: the order the draw's interval bounds are defined in
+  float before = 0.f, total = 0.f;
+#pragma unroll
+  for (int w = 0; w < kRowWarps; ++w) {
+    if (w < (tid >> 5)) before += sh_scan[w];
+    total += sh_scan[w];
+  }
+  const float hi = before + inc, lo = hi - mass_t;
+  const float target = u * total;
+  int pick = -1;
+  if ((target >= lo && target < hi && mass_t > 0.f) || (tid == kRowThreads - 1 && target >= hi)) {
+    float acc = lo;
+    pick = i1 - 1;
+    for (int i = i0; i < i1; ++i) {
+      acc += mass(i);
+      if (target < acc) { pick = i; break; }
+    }
+  }
+  *total_out = total;
+  return block_reduce_max_int(pick, sh_pick);
+}
+
+// Row `row` of the step-logits dump [steps, rows_total, V] at step `step`, or null when there is no dump.
+__device__ __forceinline__ float* step_logits_row(float* dump, int step, int rows_total, int row, int V) {
+  return dump != nullptr ? dump + (static_cast<long long>(step) * rows_total + row) * V : nullptr;
+}
+
+// Pairwise merge of two online-softmax partials (max, sum exp(x - max), arg max); an empty partial has max -inf, and the
+// lowest index wins exact ties of the maximum.
+__device__ __forceinline__ void merge_stats(float& m, float& s, int& a, float m_o, float s_o, int a_o) {
+  const float mn = fmaxf(m, m_o);
+  const float sa = (m == -INFINITY) ? 0.f : __expf(m - mn);
+  const float sb = (m_o == -INFINITY) ? 0.f : __expf(m_o - mn);
+  s = s * sa + s_o * sb;
+  if (m_o > m || (m_o == m && a_o < a)) a = a_o;
+  m = mn;
+}
+
+// The close of decode step `step`, run by the one thread that commits a unit (a row in greedy, an image in beam search)
+// after the unit's writes: the unit counts in StepState::live when it is still live, then draws one of the n_units
+// tickets.  The last ticket resets the counters, advances the loop state, stops the search when no unit is live or
+// max_steps is reached, and calls last(live count) before its closing fence.
+template <class Last>
+__device__ __forceinline__ void close_step(StepState* st, bool live, int n_units, int step, int cur_len, int max_steps,
+                                           Last last) {
+  // count this unit BEFORE drawing the ticket: the thread that draws the last ticket then sees every add
+  if (live) atomicAdd(&st->live, 1);
+  __threadfence();
+  const unsigned int t = atomicAdd(&st->ticket, 1u);
+  if (t == static_cast<unsigned int>(n_units) - 1) {
+    __threadfence();
+    const int n_live = atomicAdd(&st->live, 0);
+    st->ticket = 0;
+    st->live = 0;
+    st->cur_len = cur_len + 1;
+    st->final_len = cur_len + 1;
+    st->pos = st->pos + 1;
+    st->step = step + 1;
+    if (n_live == 0) st->finished = 1;
+    last(n_live);
+    if (cur_len + 1 >= max_steps) st->finished = 1;
+    __threadfence();
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Greedy selection = the body of AutoRegressiveBeamSearch.search for beam 1 / per-node 1
 // (reference layers/decoder.py:258-273 first step, :313-417 loop): no-repeat scatter(-10000) on the
 // input token (not on the first step), EOS forcing, log_softmax, argmax (lowest index on exact ties),
@@ -546,17 +680,6 @@ struct SelectParams {
   unsigned int* row_ticket; // [rows]
   ChainSync chain;          // last kernel of the chain: waits, then re-zeroes all counters when the step is over
 };
-
-// Pairwise merge of two online-softmax partials (max, sum exp(x - max), arg max); an empty partial has max -inf, and the
-// lowest index wins exact ties of the maximum.
-__device__ __forceinline__ void merge_stats(float& m, float& s, int& a, float m_o, float s_o, int a_o) {
-  const float mn = fmaxf(m, m_o);
-  const float sa = (m == -INFINITY) ? 0.f : __expf(m - mn);
-  const float sb = (m_o == -INFINITY) ? 0.f : __expf(m_o - mn);
-  s = s * sa + s_o * sb;
-  if (m_o > m || (m_o == m && a_o < a)) a = a_o;
-  m = mn;
-}
 
 // Where row `row` of the launch stands at this step.  in_prefix: it is still fed its prefix.  first: its first real
 // decision (no no-repeat mask).  done: it ended, its input token is EOS (reference :347-351: one-hot EOS distribution).
@@ -593,51 +716,29 @@ __device__ __forceinline__ RowChoice resolve_row(const SelectParams& p, int row,
   return c;
 }
 
-// Commits one row's choice; the row that draws the step's last ticket advances the loop state (the reference stops once
-// every token it feeds next is EOS) and re-zeroes the chain counters (null: none).
+// Commits one row's choice and closes the step with it: a row is live while the token it feeds next is not EOS (the
+// reference stops once every one is).  The last ticket also marks an empty caption and re-zeroes the chain counters
+// (null: none).
 __device__ __forceinline__ void commit_row(const SelectParams& p, int row, int step, int cur_len, const RowChoice& c,
                                            unsigned int* chain_counters) {
-  StepState* st = p.state;
   p.tokens_out[static_cast<long long>(row) * p.max_steps + cur_len] = c.tok;
   p.logprob_sum[row] += c.lp;
   p.next_token[row] = c.nxt;
-  if (c.nxt != p.eos) atomicAdd(&st->not_eos, 1);
-  __threadfence();
-  const unsigned int tr = atomicAdd(&st->ticket, 1u);
-  if (tr == static_cast<unsigned int>(p.rows) - 1) {
-    __threadfence();
-    const int not_eos = atomicAdd(&st->not_eos, 0);
-    st->ticket = 0;
-    st->not_eos = 0;
-    st->cur_len = cur_len + 1;
-    st->final_len = cur_len + 1;
-    st->pos = st->pos + 1;
-    st->step = step + 1;
-    if (not_eos == 0) {
-      st->finished = 1;
-      if (step == 0 && p.row_prefix == nullptr) st->empty_caption = 1;
-    }
-    if (cur_len + 1 >= p.max_steps) st->finished = 1;
+  close_step(p.state, c.nxt != p.eos, p.rows, step, cur_len, p.max_steps, [&](int n_live) {
+    if (n_live == 0 && step == 0 && p.row_prefix == nullptr) p.state->empty_caption = 1;
     // every CTA of every kernel of this step has passed its wait: recycle the chain counters
     if (chain_counters != nullptr)
       for (int k = 0; k < 64; ++k) chain_counters[k] = 0;
-    __threadfence();
-  }
+  });
 }
 
 // grid (n_split, rows): each CTA folds one vocabulary slice of one row into (max, argmax, sum exp) with a
 // single online pass; the last CTA of a row combines the slices and does the reference's bookkeeping.
-__global__ void __launch_bounds__(256) greedy_select_kernel(const SelectParams p) {
+__global__ void __launch_bounds__(kRowThreads) greedy_select_kernel(const SelectParams p) {
   griddep_launch_early();
   tl_mark(100005);
   StepState* st = p.state;
-  if (p.chain.counters != nullptr) {
-    if (st->finished) return;  // stable within a step
-    chain_wait(p.chain);
-  } else {
-    griddep_wait();
-    if (st->finished) return;
-  }
+  if (step_wait(&st->finished, p.chain)) return;
   tl_mark(5);
   const int row = blockIdx.y;
   const int split = blockIdx.x;
@@ -652,23 +753,21 @@ __global__ void __launch_bounds__(256) greedy_select_kernel(const SelectParams p
   const int chunk = (p.V + p.n_split - 1) / p.n_split;
   const int lo = split * chunk;
   const int hi = min(p.V, lo + chunk);
-  if (p.step_logits != nullptr) {
-    float* dst = p.step_logits + (static_cast<long long>(step) * p.rows_total + p.row0 + row) * p.V;
-    for (int i = lo + tid; i < hi; i += 256) dst[i] = z[i];
-  }
+  if (float* dst = step_logits_row(p.step_logits, step, p.rows_total, p.row0 + row, p.V))
+    for (int i = lo + tid; i < hi; i += kRowThreads) dst[i] = z[i];
   float m = -INFINITY, ssum = 0.f;
   int arg = 0x7fffffff;
-  for (int i0 = lo + tid; i0 < hi; i0 += 16 * 256) {   // one round for the usual 8-way split of 30522
+  for (int i0 = lo + tid; i0 < hi; i0 += 16 * kRowThreads) {   // one round for the usual 8-way split of 30522
     float v[16];
 #pragma unroll
     for (int u = 0; u < 16; ++u) {
-      const int i = i0 + u * 256;
+      const int i = i0 + u * kRowThreads;
       v[u] = (i < hi) ? __ldcg(z + i) : -INFINITY;
       if (!rs.first && i == static_cast<int>(last)) v[u] = -10000.0f;   // no-repeat (reference :330)
     }
 #pragma unroll
     for (int u = 0; u < 16; ++u) {
-      const int i = i0 + u * 256;
+      const int i = i0 + u * kRowThreads;
       if (v[u] > m) {   // increasing i per thread: keeps the lowest index on exact ties
         ssum = ssum * __expf(m - v[u]) + 1.0f;
         m = v[u];
@@ -679,8 +778,8 @@ __global__ void __launch_bounds__(256) greedy_select_kernel(const SelectParams p
     }
   }
   // block reduce of (m, arg, ssum)
-  __shared__ float s_m[8], s_s[8];
-  __shared__ int s_a[8];
+  __shared__ float s_m[kRowWarps], s_s[kRowWarps];
+  __shared__ int s_a[kRowWarps];
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1)
     merge_stats(m, ssum, arg, __shfl_xor_sync(0xffffffffu, m, o), __shfl_xor_sync(0xffffffffu, ssum, o),
@@ -688,7 +787,7 @@ __global__ void __launch_bounds__(256) greedy_select_kernel(const SelectParams p
   if ((tid & 31) == 0) { s_m[tid >> 5] = m; s_s[tid >> 5] = ssum; s_a[tid >> 5] = arg; }
   __syncthreads();
   if (tid == 0) {
-    for (int w = 1; w < 8; ++w) merge_stats(m, ssum, arg, s_m[w], s_s[w], s_a[w]);
+    for (int w = 1; w < kRowWarps; ++w) merge_stats(m, ssum, arg, s_m[w], s_s[w], s_a[w]);
     p.part_max[row * p.n_split + split] = m;
     p.part_sum[row * p.n_split + split] = ssum;
     p.part_arg[row * p.n_split + split] = arg;

@@ -12,13 +12,14 @@
 //   beam_finalize_kernel : decoded[B, max_steps] (EOS padded) and the length-normalised score.
 // The text KV cache is never copied: src_row[r][j] names the physical row that holds position j of
 // logical row r's history.
+// The per-row kernels (and beam_sample_kernel below) use the CTA reductions, the inverse-CDF lookup and the step-logits
+// row of rowops.cuh; beam_update_kernel closes each step with close_step there, as the greedy kernels do.
 //
 // Candidate order: (score desc, beam asc, logit desc, token asc).  A row's list is ranked on the raw logit (lower token on
 // exact ties); the score ((z - max) - log_sum) + beam_score is increasing in z in exact arithmetic, but fp32 can round two
 // different logits of one row to the same score (e.g. z - max = -100 for a logit one ulp apart), and those keep the logit
 // order -- the order of their exact scores.  The merge breaks equal scores of different beams by the lower flat index.
 #pragma once
-#include "constrained.cuh"
 #include "ptx.cuh"
 #include "rowops.cuh"
 
@@ -111,34 +112,33 @@ struct TopList {
 
 // One CTA per row: lse = logsumexp(z), then the row's top-NC values of (z - lse + beam_score[row]).  One pass over the
 // logits (online max / sum-exp and a sorted top-8 list per thread), then lists merged by shuffles and through shared memory.
-__global__ void __launch_bounds__(256) beam_row_topk_kernel(const BeamParams p) {
+__global__ void __launch_bounds__(kRowThreads) beam_row_topk_kernel(const BeamParams p) {
   griddep_launch();
-  griddep_wait();
   StepState* st = p.state;
-  if (st->finished) return;
+  if (step_wait(&st->finished, ChainSync{})) return;
   const int row = blockIdx.x;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int NC = p.per_node * p.beam;
   const float* z = p.logits + static_cast<long long>(row) * p.V;
-  if (p.step_logits != nullptr) {
-    float* dst = p.step_logits + (static_cast<long long>(st->step) * gridDim.x + row) * p.V;
-    for (int i = tid; i < p.V; i += blockDim.x) dst[i] = z[i];
-  }
+  if (float* dst = step_logits_row(p.step_logits, st->step, gridDim.x, row, p.V))
+    for (int i = tid; i < p.V; i += blockDim.x) dst[i] = z[i];   // a kRowThreads stride changes the kernel's code
   TopList top;
   top.init();
   float mx = -INFINITY, sum = 0.f;
-  for (int i0 = tid; i0 < p.V; i0 += 8 * 256) {       // 8 independent loads in flight per thread
+  for (int i0 = tid; i0 < p.V; i0 += 8 * kRowThreads) {       // 8 independent loads in flight per thread
     float v[8];
 #pragma unroll
-    for (int u = 0; u < 8; ++u) v[u] = (i0 + u * 256 < p.V) ? __ldcg(z + i0 + u * 256) : -INFINITY;
+    for (int u = 0; u < 8; ++u) v[u] = (i0 + u * kRowThreads < p.V) ? __ldcg(z + i0 + u * kRowThreads) : -INFINITY;
 #pragma unroll
     for (int u = 0; u < 8; ++u) {
       if (v[u] == -INFINITY) continue;
       if (v[u] > mx) { sum = sum * __expf(mx - v[u]) + 1.0f; mx = v[u]; } else { sum += __expf(v[u] - mx); }
-      top.push(v[u], i0 + u * 256);
+      top.push(v[u], i0 + u * kRowThreads);
     }
   }
-  // warp-level merge: each round a lane absorbs its partner's list (entries arrive in sorted order: push keeps ours sorted)
+  // warp-level merge: each round a lane absorbs its partner's list (entries arrive in sorted order: push keeps ours sorted).
+  // The (max, sum exp) merges here are merge_stats without the arg max, written out: a shared helper for them changed the
+  // kernel's register allocation (62 -> 48 or 64 registers) and left the deterministic beam step slower.
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) {
     const float m_o = __shfl_xor_sync(0xffffffffu, mx, o);
@@ -153,9 +153,9 @@ __global__ void __launch_bounds__(256) beam_row_topk_kernel(const BeamParams p) 
 #pragma unroll
     for (int k = 0; k < kMaxCand; ++k) top.push(pv[k], pi[k]);
   }
-  __shared__ float s_m[8], s_s[8];
-  __shared__ float s_cv[8][kMaxCand];
-  __shared__ int s_ci[8][kMaxCand];
+  __shared__ float s_m[kRowWarps], s_s[kRowWarps];
+  __shared__ float s_cv[kRowWarps][kMaxCand];
+  __shared__ int s_ci[kRowWarps][kMaxCand];
   if (lane == 0) {
     s_m[warp] = mx; s_s[warp] = sum;
 #pragma unroll
@@ -163,7 +163,7 @@ __global__ void __launch_bounds__(256) beam_row_topk_kernel(const BeamParams p) 
   }
   __syncthreads();
   if (tid == 0) {
-    for (int w = 1; w < 8; ++w) {
+    for (int w = 1; w < kRowWarps; ++w) {
       const float mn = fmaxf(mx, s_m[w]);
       sum = sum * ((mx == -INFINITY) ? 0.f : __expf(mx - mn)) + s_s[w] * ((s_m[w] == -INFINITY) ? 0.f : __expf(s_m[w] - mn));
       mx = mn;
@@ -202,31 +202,14 @@ __device__ __forceinline__ float key_value(unsigned int k) {
   return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
 }
 
-__device__ __forceinline__ int block_exclusive_scan_int(int v, int* sh) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int inc = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int up = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += up;
-  }
-  if (lane == 31) sh[warp] = inc;
-  __syncthreads();
-  int before = 0;
-#pragma unroll
-  for (int w = 0; w < 8; ++w) if (w < warp) before += sh[w];
-  __syncthreads();
-  return before + inc - v;
-}
-
 struct SampleSmem {
-  int cnt[8][256];      // per-warp digit histograms: counts ...
-  float mass[8][256];   // ... and masses
-  float stage[8][32];
-  int scan_c[256];      // inclusive scans over the buckets, in descending key order
+  int cnt[kRowWarps][256];      // per-warp digit histograms: counts ...
+  float mass[kRowWarps][256];   // ... and masses
+  float stage[kRowWarps][32];
+  int scan_c[256];              // inclusive scans over the buckets, in descending key order
   float scan_m[256];
-  float red[8];
-  int ired[8];
+  float red[kRowWarps];
+  int ired[kRowWarps];
 };
 
 // Where a descending walk over the keys stops: the key, how many keys lie strictly above it (and their mass), how many
@@ -248,6 +231,7 @@ struct RadixStop {
 // buckets need not add up to the total the pass before saw), the descent takes the lowest non-empty bucket.
 template <bool kMass>
 __device__ RadixStop radix_descend(const float* s, int V, float want, unsigned int live, float m, SampleSmem& sm) {
+  static_assert(kRowThreads == 256, "one thread per 8-bit digit bucket");
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   RadixStop r{0u, 0, 0, 0.f, true};
   unsigned int mask = 0u;
@@ -257,7 +241,7 @@ __device__ RadixStop radix_descend(const float* s, int V, float want, unsigned i
       if (kMass) sm.mass[warp][d] = 0.f;
     }
     __syncwarp();
-    for (int base = 0; base < V; base += 256) {
+    for (int base = 0; base < V; base += kRowThreads) {
       const int i = base + tid;
       unsigned int key = 0u;
       bool in = false;
@@ -287,29 +271,26 @@ __device__ RadixStop radix_descend(const float* s, int V, float want, unsigned i
     int c = 0;
     float ms = 0.f;
 #pragma unroll
-    for (int w = 0; w < 8; ++w) {
+    for (int w = 0; w < kRowWarps; ++w) {
       c += sm.cnt[w][d];
       if (kMass) ms += sm.mass[w][d];
     }
-    int ci = c;
-    float mi = ms;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int cu = __shfl_up_sync(0xffffffffu, ci, o);
-      const float mu = __shfl_up_sync(0xffffffffu, mi, o);
-      if (lane >= o) { ci += cu; mi += mu; }
-    }
+    int ci = warp_inclusive_scan(c);
+    float mi = kMass ? warp_inclusive_scan(ms) : 0.f;
     if (lane == 31) { sm.ired[warp] = ci; sm.red[warp] = mi; }
     __syncthreads();
+    // ((inc + t_0) + t_1) + ...: the order the masses above a bucket are defined in
 #pragma unroll
-    for (int w = 0; w < 8; ++w) {
+    for (int w = 0; w < kRowWarps; ++w) {
       if (w < warp) { ci += sm.ired[w]; if (kMass) mi += sm.red[w]; }
     }
     __syncthreads();
     sm.scan_c[tid] = ci;
     if (kMass) sm.scan_m[tid] = mi;
     const bool stop = kMass ? (c > 0 && r.mass_above + mi > want) : (static_cast<float>(r.above + ci) >= want);
-    int t = 255 - block_reduce_max_int(stop ? 255 - tid : -1, sm.ired);   // the first bucket that stops (256: none)
+    // the first bucket that stops (256: none); as a max of 255 - t: block_reduce_min_int here made ptxas give the kernel
+    // 46 registers instead of 39
+    int t = 255 - block_reduce_max_int(stop ? 255 - tid : -1, sm.ired);
     if (t > 255) {
       if (kMass && shift == 24) { r.found = false; return r; }
       t = block_reduce_max_int(c > 0 ? tid : -1, sm.ired);
@@ -325,25 +306,24 @@ __device__ RadixStop radix_descend(const float* s, int V, float want, unsigned i
   return r;
 }
 
-__global__ void __launch_bounds__(256) beam_sample_kernel(const BeamParams p) {
+__global__ void __launch_bounds__(kRowThreads) beam_sample_kernel(const BeamParams p) {
   griddep_launch();
-  griddep_wait();
   StepState* st = p.state;
-  if (st->finished) return;
+  if (step_wait(&st->finished, ChainSync{})) return;
   extern __shared__ float srow[];   // the row's scores logits / T
   __shared__ SampleSmem sm;
   const int row = blockIdx.x, rows = gridDim.x, tid = threadIdx.x, V = p.V;
   const int cur_len = st->cur_len;
   const float* z = p.logits + static_cast<long long>(row) * V;
-  float* dump = p.step_logits != nullptr ? p.step_logits + (static_cast<long long>(st->step) * rows + row) * V : nullptr;
+  float* dump = step_logits_row(p.step_logits, st->step, rows, row, V);
   float mx = -INFINITY;
-  for (int i0 = tid; i0 < V; i0 += 8 * 256) {        // 8 independent loads in flight per thread
+  for (int i0 = tid; i0 < V; i0 += 8 * kRowThreads) {        // 8 independent loads in flight per thread
     float v[8];
 #pragma unroll
-    for (int k = 0; k < 8; ++k) v[k] = (i0 + k * 256 < V) ? __ldcg(z + i0 + k * 256) : 0.f;
+    for (int k = 0; k < 8; ++k) v[k] = (i0 + k * kRowThreads < V) ? __ldcg(z + i0 + k * kRowThreads) : 0.f;
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
-      const int i = i0 + k * 256;
+      const int i = i0 + k * kRowThreads;
       if (i >= V) break;
       if (dump != nullptr) dump[i] = v[k];
       const float sv = v[k] / p.smp.temperature;   // a division, as the reference: a multiply by 1/T can split a tie it makes
@@ -369,7 +349,7 @@ __global__ void __launch_bounds__(256) beam_sample_kernel(const BeamParams p) {
   const float top_p = p.smp.top_p;
   if (top_p != 0.f && top_p < 1.f) {
     float w = 0.f;
-    for (int i = tid; i < V; i += 256)
+    for (int i = tid; i < V; i += kRowThreads)
       if (order_key(srow[i]) >= live) w += expf(srow[i] - m);
     const float target = top_p * block_reduce_sum(w, sm.red);   // cumsum(softmax) > p  <=>  cumsum(exp(s - m)) > p * sum
     const RadixStop c = radix_descend<true>(srow, V, target, live, m, sm);
@@ -395,7 +375,7 @@ __global__ void __launch_bounds__(256) beam_sample_kernel(const BeamParams p) {
     }
   }
   // thread t owns the contiguous indices [i0, i1): ties and draws go in index order (an odd stride: no bank conflicts)
-  const int C = ((V + 255) / 256) | 1;
+  const int C = ((V + kRowThreads - 1) / kRowThreads) | 1;
   const int i0 = min(V, tid * C), i1 = min(V, i0 + C);
   int i_last = V;
   if (keep_ties != 0x7fffffff) {
@@ -462,9 +442,8 @@ __global__ void __launch_bounds__(256) beam_sample_kernel(const BeamParams p) {
 // One thread block per image (32 threads; the bookkeeping itself is sequential like the reference's loop).
 __global__ void __launch_bounds__(32) beam_update_kernel(const BeamParams p) {
   griddep_launch();
-  griddep_wait();
   StepState* st = p.state;
-  if (st->finished) return;
+  if (step_wait(&st->finished, ChainSync{})) return;
   const int b = blockIdx.x;
   const int lane = threadIdx.x;
   const int beam = p.beam, NC = p.per_node * p.beam, V = p.V;
@@ -582,27 +561,10 @@ __global__ void __launch_bounds__(32) beam_update_kernel(const BeamParams p) {
       p.s.beam_scores[r] = n_score[k];
     }
   }
-  // loop-state advance by the last image
+  // loop-state advance by the last image: an image is live until it is done, and the search stops once every image is
+  // (`if all(done): break`, :1253)
   __threadfence();
-  if (lane == 0) {
-    // count this image as running BEFORE drawing the ticket: the block that draws the last ticket then sees every add
-    if (p.s.done[b] == 0) atomicAdd(&st->not_eos, 1);  // re-used as "images still running"
-    __threadfence();
-    const unsigned int t = atomicAdd(&st->ticket, 1u);
-    if (t == static_cast<unsigned int>(p.B) - 1) {
-      __threadfence();
-      const int running = atomicAdd(&st->not_eos, 0);
-      st->ticket = 0;
-      st->not_eos = 0;
-      *p.s.cur = cur ^ 1;
-      st->cur_len = cur_len + 1;
-      st->final_len = cur_len + 1;
-      st->pos = st->pos + 1;
-      st->step = st->step + 1;
-      if (running == 0 || cur_len + 1 >= p.max_steps) st->finished = 1;  // `if all(done): break` (:1253)
-      __threadfence();
-    }
-  }
+  if (lane == 0) close_step(st, p.s.done[b] == 0, p.B, st->step, cur_len, p.max_steps, [&](int) { *p.s.cur = cur ^ 1; });
 }
 
 __global__ void beam_init_kernel(BeamState s, long long* next_token, const long long* prefix, int P, int sos, int B,
