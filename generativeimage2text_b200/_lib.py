@@ -5,7 +5,7 @@ import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, 'libgitb200.so')
-ABI_VERSION = 11
+ABI_VERSION = 12
 
 c_void_p, c_int, c_int64, c_float, c_char_p = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_char_p
 c_ll = ctypes.c_longlong
@@ -69,6 +69,7 @@ SIGNATURES = {
     'gitb200_set_trie': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int]),
     'gitb200_set_sampling': (c_int, [c_void_p, c_void_p, c_int, c_int, c_float]),
     'gitb200_set_beam_sampling': (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_int, c_float]),
+    'gitb200_set_sequences_per_image': (c_int, [c_void_p, c_int]),
     'gitb200_launch_count': (c_int64, [c_void_p]),
     'gitb200_set_option': (c_int, [c_void_p, c_char_p, c_int64]),
     'gitb200_preproc_create': (c_int, [c_int, ctypes.POINTER(c_void_p)]),

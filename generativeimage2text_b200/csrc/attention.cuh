@@ -304,7 +304,8 @@ struct DecAttnParams {
   __nv_bfloat16* txt_v;
   const int* src_row;              // [R, T_alloc] physical row holding text position j of logical row r (null = r)
   __nv_bfloat16* ctx;              // [R, D]
-  int B, M, T_alloc, D;
+  int B, M, T_alloc, D;            // B: sequence groups of NQ rows each (R = B * NQ)
+  int seqs_per_image;              // groups that share one image's K/V: group b reads image b / seqs_per_image
   const StepState* state;          // text position = state->pos (or pos_fixed when null)
   int pos_fixed;
   int chunk_rows;                  // image keys staged per TMA round (<= 512), box_rows * n_boxes
@@ -398,7 +399,7 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
   if constexpr (kRagged) {
     n_units = 0;
     for (int k = 0; k < n_my; ++k) {
-      const int Mb = p.img_lens[(static_cast<int>(blockIdx.x) + k * G) / H];
+      const int Mb = p.img_lens[(static_cast<int>(blockIdx.x) + k * G) / H / p.seqs_per_image];
       n_units += (Mb + dec_attn_chunk_rows(Mb) - 1) / dec_attn_chunk_rows(Mb);
     }
   }
@@ -419,16 +420,17 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
     const int c = kRagged ? iss_c : u - k * n_chunks;
     const int item = blockIdx.x + k * G;
     const int b = item / H, h = item - b * H;
+    const int img = b / p.seqs_per_image;
     uint8_t* sK = sbase + static_cast<size_t>(u & 1) * 2 * kv_bytes;
     uint8_t* sV = sK + kv_bytes;
-    const int Mb = kRagged ? p.img_lens[b] : p.M;
+    const int Mb = kRagged ? p.img_lens[img] : p.M;
     const int crows = kRagged ? dec_attn_chunk_rows(Mb) : p.chunk_rows;
     const int box = kRagged ? kDecAttnRaggedBox : p.box_rows;
     const int rows_c = min(crows, Mb - c * crows);
     const int nb = (rows_c + box - 1) / box;
     mbar_arrive_expect_tx(&bars[u & 1], static_cast<uint32_t>(2 * nb * box * 128));
     for (int i = 0; i < nb; ++i) {
-      const int grow = b * p.M + c * crows + i * box;
+      const int grow = img * p.M + c * crows + i * box;
       const int gcol = h * 64;
       tma_load_2d(sK + static_cast<size_t>(i) * box * 128, &tmK, &bars[u & 1], gcol, grow);
       tma_load_2d(sV + static_cast<size_t>(i) * box * 128, &tmV, &bars[u & 1], gcol, grow);
@@ -495,7 +497,7 @@ decode_attn_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
   for (int k = 0; k < n_my; ++k) {
     const int item = blockIdx.x + k * G;
     const int b = item / H, h = item - b * H;
-    const int Mb = kRagged ? p.img_lens[b] : p.M;
+    const int Mb = kRagged ? p.img_lens[b / p.seqs_per_image] : p.M;
     const int crows = kRagged ? dec_attn_chunk_rows(Mb) : p.chunk_rows;
     const int nch = kRagged ? (Mb + crows - 1) / crows : n_chunks;
     float cur_a = 0.f, cur_b = 0.f;
@@ -811,7 +813,7 @@ struct DecAttnF32Params {
   float* txt_v;
   const int* src_row;
   __nv_bfloat16* ctx;             // split3 rows [R, 3 * D]
-  int R, beam, M, T_alloc, D;
+  int R, rows_per_image, M, T_alloc, D;   // row r reads image r / rows_per_image (sequences per image x beam)
   const StepState* state;
   int pos_fixed;
   ChainSync chain;
@@ -836,7 +838,7 @@ __global__ void __launch_bounds__(128) decode_attn_f32_kernel(const DecAttnF32Pa
   const int item = blockIdx.x * 4 + warp;
   if (item < p.R * H) {
     const int r = item / H, h = item - r * H;
-    const int b = r / p.beam;
+    const int b = r / p.rows_per_image;
     const int Mb = p.img_lens != nullptr ? p.img_lens[b] : p.M;
     const int n_keys = Mb + pos + 1;
     const float* row = p.qkv + static_cast<long long>(r) * 3 * D + h * 64;

@@ -45,7 +45,7 @@
 using namespace gitb200;
 typedef __nv_bfloat16 bf16;
 
-#define GITB200_ABI_VERSION 11
+#define GITB200_ABI_VERSION 12
 
 // ------------------------------------------------------------------------------------------------
 // errors
@@ -189,6 +189,7 @@ struct gitb200_engine {
   DevBuf chain;                                             // decode-step kernel chain completion counters [64]
   DecAttnGeom attn_geom{};                                  // decode_attn_kernel geometry of the last prefill
   int cur_B = 0, cur_frames = 0, cur_M = 0, cur_beam = 1, T_alloc = 0, cur_rows = 0, cur_src = 0;
+  int cur_seqs = 1;                                         // sequences per image of the last prefill (rows = B * seqs * beam)
 
   EncodeTiledFn encode_tiled = nullptr;
   std::map<TmapKey, CUtensorMap> tmaps;
@@ -229,6 +230,7 @@ struct gitb200_engine {
     int beam_sample_steps = 0, beam_sample_rows = 0;
     float beam_temperature = 1.0f, beam_top_p = 1.0f;
     int beam_top_k = 0;
+    int seqs_per_image = 1;               // gitb200_set_sequences_per_image
   } next;
 };
 
@@ -664,10 +666,11 @@ static int launch_decode_attn_inst(gitb200_engine* h, const DecAttnParams& ap, i
   return 0;
 }
 
-// Decode-step attention (attention.cuh) of B images x beam rows at one text position (state->pos, or pos_fixed when state
+// Decode-step attention (attention.cuh) of B images x seqs sequences x beam rows at one text position (state->pos, or pos_fixed when state
 // is null): adds the QKV GEMM's n_partials split-K buffers and the bias, appends k / v to the text cache [R, T_alloc, D]
 // (rows through src_row when non-null) and attends to the image K/V [B, M, D] (img_lens: null, or [B] valid keys) and the
-// text keys so far.  bf16: decode_attn_kernel<beam, ragged> with geom from dec_attn_geometry.  fp32 (parity mode):
+// text keys so far; the seqs sequences of an image (row groups of beam rows) read its one image K/V.  bf16:
+// decode_attn_kernel<beam, ragged> over B * seqs groups, with geom from dec_attn_geometry.  fp32 (parity mode):
 // decode_attn_f32_kernel, one warp per (row, head), ctx rows [hi | lo | hi].  *ctas receives the grid.
 struct DecodeAttn {
   const float* qkv;
@@ -679,7 +682,7 @@ struct DecodeAttn {
   void* txt_v;
   const int* src_row;
   bf16* ctx;
-  int B, beam, M, T_alloc, D;
+  int B, seqs, beam, M, T_alloc, D;
   const StepState* state;
   int pos_fixed;
   const int* img_lens;
@@ -688,14 +691,14 @@ struct DecodeAttn {
   bool pdl;
 };
 static int launch_decode_attention(gitb200_engine* h, const DecodeAttn& a, bool fp32, cudaStream_t st, unsigned int* ctas) {
-  const int R = a.B * a.beam;
+  const int R = a.B * a.seqs * a.beam;
   if (fp32) {
     DecAttnF32Params p{};
     p.qkv = a.qkv; p.n_partials = a.n_partials; p.partial_stride = static_cast<long long>(R) * 3 * a.D;
     p.bqkv = a.bqkv;
     p.img_k = static_cast<const float*>(a.img_k); p.img_v = static_cast<const float*>(a.img_v);
     p.txt_k = static_cast<float*>(a.txt_k); p.txt_v = static_cast<float*>(a.txt_v);
-    p.src_row = a.src_row; p.ctx = a.ctx; p.R = R; p.beam = a.beam; p.M = a.M; p.T_alloc = a.T_alloc; p.D = a.D;
+    p.src_row = a.src_row; p.ctx = a.ctx; p.R = R; p.rows_per_image = a.seqs * a.beam; p.M = a.M; p.T_alloc = a.T_alloc; p.D = a.D;
     p.state = a.state; p.pos_fixed = a.pos_fixed;
     p.chain = a.chain;
     p.img_lens = a.img_lens;
@@ -712,7 +715,7 @@ static int launch_decode_attention(gitb200_engine* h, const DecodeAttn& a, bool 
   p.bqkv = a.bqkv;
   p.img_k = static_cast<const bf16*>(a.img_k); p.img_v = static_cast<const bf16*>(a.img_v);
   p.txt_k = static_cast<bf16*>(a.txt_k); p.txt_v = static_cast<bf16*>(a.txt_v);
-  p.src_row = a.src_row; p.ctx = a.ctx; p.B = a.B; p.M = a.M; p.T_alloc = a.T_alloc; p.D = a.D;
+  p.src_row = a.src_row; p.ctx = a.ctx; p.B = a.B * a.seqs; p.seqs_per_image = a.seqs; p.M = a.M; p.T_alloc = a.T_alloc; p.D = a.D;
   p.state = a.state; p.pos_fixed = a.pos_fixed;
   p.chunk_rows = a.geom.chunk_rows; p.box_rows = a.geom.box_rows;
   p.chain = a.chain;
@@ -1392,10 +1395,11 @@ static int image_rows(gitb200_engine* h, float* vproj_out, cudaStream_t st) {
   return decoder_layers(h, rows, h->img_kv.as<char>(), true, true, self_attention, st);
 }
 
-static int prefill_impl(gitb200_engine* h, int B, int beam, int T_alloc, float* vproj_out, cudaStream_t st) {
+// Sizes the decode step for B images x seqs sequences x beam rows; the image K/V cache holds the B images once.
+static int prefill_impl(gitb200_engine* h, int B, int seqs, int beam, int T_alloc, float* vproj_out, cudaStream_t st) {
   if (B != h->cur_B || h->cur_M <= 0) return fail(h, "prefill: call encode with the same batch first");
   const int D = h->D, F = h->F, nl = h->cfg.dec_layers;
-  const int R = B * beam;
+  const int R = B * seqs * beam;
   const int ks = h->ks();
   const long long kvb = static_cast<long long>(h->kvb());
   TRY(decoder_buffers(h, 0));
@@ -1425,6 +1429,7 @@ static int prefill_impl(gitb200_engine* h, int B, int beam, int T_alloc, float* 
   CK(h->next_token.ensure(static_cast<size_t>(R) * 8));
   CK(h->logprob_sum.ensure(static_cast<size_t>(R) * 4));
   h->cur_beam = beam;
+  h->cur_seqs = seqs;
   h->cur_rows = R;
   h->T_alloc = T_alloc;
   return image_rows(h, vproj_out, st);
@@ -1484,7 +1489,7 @@ static int step_layers(gitb200_engine* h, cudaStream_t st, const long long* toke
   DecodeAttn da{};
   da.n_partials = kQkvSplits;
   da.src_row = src_row; da.ctx = ctx;
-  da.B = h->cur_B; da.beam = beam; da.M = h->cur_M; da.T_alloc = h->T_alloc; da.D = D;
+  da.B = h->cur_B; da.seqs = h->cur_seqs; da.beam = beam; da.M = h->cur_M; da.T_alloc = h->T_alloc; da.D = D;
   da.state = state;
   da.img_lens = img_lens(h, h->cur_img);
   da.geom = h->attn_geom;
@@ -1524,7 +1529,7 @@ static int step_layers(gitb200_engine* h, cudaStream_t st, const long long* toke
 // Decode-attention geometry of the last prefill (dec_attn_geometry) and the step chain's counters.
 static int set_decode_geometry(gitb200_engine* h) {
   h->attn_geom = dec_attn_geometry(h->cur_M, h->cur_img.ragged ? h->cur_img.lens.data() : nullptr, h->cur_B, h->num_sms,
-                                   h->cur_B * h->cfg.dec_heads);
+                                   h->cur_B * h->cur_seqs * h->cfg.dec_heads);
   CK(h->chain.ensure(256));
   CK(cudaMemset(h->chain.p, 0, 256));
   return 0;

@@ -10,6 +10,7 @@ storage, the CUDA stream and the output tensors.
 """
 import collections
 import ctypes
+import numbers
 import warnings
 
 import torch
@@ -510,8 +511,14 @@ class GitB200CaptioningModel(nn.Module):
                accepted and ignored exactly like the reference (its filter call is commented out, :372) -- plus
                'uniforms': FloatTensor[max_steps, B] or 'generator': torch.Generator for the random numbers;
                {'do_sample': True, 'top_k': int, 'top_p': .} with GeneratorWithBeamSearch (the temperature is the
-               decoder's `temperature` attribute; num_keep_best / num_return_sequences only 1) plus 'uniforms': FloatTensor[max_steps,
-               B * beam_size, 2] or 'generator'.
+               decoder's `temperature` attribute; num_keep_best only 1) plus 'uniforms': FloatTensor[max_steps,
+               B * beam_size, 2] or 'generator';
+               'num_return_sequences': n (an int >= 1, every decoder): B images give B * n sequences in image-major order
+               (row b * n + i belongs to image b; per-image prefixes apply to all n), each searching on its own, and every
+               B above counts sequences: 'uniforms' [max_steps, B * n] (beam: [max_steps, B * n * beam_size, 2]),
+               forced_tokens [B * n, max_steps], predictions / logprobs / step_logits B * n (* beam) rows.  Each image is
+               encoded and its K/V cached once; the result is bit for bit that of the call with every image repeated n
+               times (greedy without sampling: with use_mega 0, since n > 1 runs on the kernel chain).
         """
         return self.submit(batch, forced_tokens, return_step_logits, slot=0, _caller_stream=True,
                            search_param=search_param).result()
@@ -532,6 +539,7 @@ class GitB200CaptioningModel(nn.Module):
         if 'context' in batch:
             raise NotImplementedError("'context' batches are not produced by the reference inference path")
         search_param = dict(search_param or {})
+        n_seq = _sequences_per_image(search_param.pop('num_return_sequences', 1))
         constrained = bool(search_param) or isinstance(self.decoder, TrieAutoRegressiveBeamSearch)
         image = batch['image']
         # (copies / casts, if any, run on the caller's stream; a coalesced group hands over its images as one _Images)
@@ -539,7 +547,7 @@ class GitB200CaptioningModel(nn.Module):
         x, B, frames = img.x, img.B, img.frames
         # a ragged batch is launched on its own (never coalesced)
         if (int(coalesce) > 1 and img.sizes is None and slot is None and not _caller_stream and forced_tokens is None and not return_step_logits
-                and 'prefix' not in batch and 'prefix_len' not in batch and not constrained):
+                and 'prefix' not in batch and 'prefix_len' not in batch and not constrained and n_seq == 1):
             return self._submit_coalesced(img, depth, int(coalesce))
         if self._open_group is not None:
             self._open_group.launch()         # keep the submission order
@@ -580,6 +588,9 @@ class GitB200CaptioningModel(nn.Module):
                 raise ValueError("'prefix_len' must hold B lengths in [1, P] below the decoder's max_steps")
             if forced_tokens is not None:
                 raise ValueError('teacher forcing is not available for per-image prefixes')
+            if n_seq > 1:           # every sequence of image b starts from image b's prefix
+                row_prefix = row_prefix.repeat_interleave(n_seq, 0)
+                row_lens = [n for n in row_lens for _ in range(n_seq)]
             row_lens_dev = torch.tensor(row_lens, dtype=torch.int32, device=dev)
         elif 'prefix' in batch:
             assert len(batch['prefix']) == 1, 'not supported'      # reference layers/decoder.py:988
@@ -587,23 +598,24 @@ class GitB200CaptioningModel(nn.Module):
                 raise AssertionError('not supported: one shared prefix needs batch size 1 (pass a [B, P] prefix for one per image)')
             prefix = batch['prefix'].to(device=dev, dtype=torch.long).contiguous().view(-1)
             P = prefix.numel()
-        tokens = torch.empty((B, sp.max_steps), dtype=torch.long, device=dev)
-        logprobs = torch.empty((B,), dtype=torch.float32, device=dev)
+        S = B * n_seq                         # sequences: row b * n_seq + i belongs to image b
+        tokens = torch.empty((S, sp.max_steps), dtype=torch.long, device=dev)
+        logprobs = torch.empty((S,), dtype=torch.float32, device=dev)
         forced = None
         if forced_tokens is not None:
             forced = forced_tokens.to(device=dev, dtype=torch.long).contiguous()
-            assert tuple(forced.shape) == (B, sp.max_steps)
+            assert tuple(forced.shape) == (S, sp.max_steps)
         step_logits = None
         if return_step_logits:
-            rows = B * (sp.beam_size if sp.mode == _lib.SEARCH_BEAM else 1)
+            rows = S * (sp.beam_size if sp.mode == _lib.SEARCH_BEAM else 1)
             step_logits = torch.zeros((sp.max_steps - max(P, 1), rows, VOCAB), dtype=torch.float32, device=dev)
-        uniforms = self._sampling_setup(search_param, sp, B, dev)
+        uniforms = self._sampling_setup(search_param, sp, S, dev)
         for t in (x, prefix, forced, row_prefix, row_lens_dev, uniforms):
             if t is not None and stream is not cur:
                 t.record_stream(stream)
         self._set_image_sizes(lib, eng, img)
         if row_prefix is not None:
-            _lib.check(lib.gitb200_set_row_prefixes(eng, row_prefix.data_ptr(), B, int(row_prefix.shape[1]), row_lens_dev.data_ptr()),
+            _lib.check(lib.gitb200_set_row_prefixes(eng, row_prefix.data_ptr(), S, int(row_prefix.shape[1]), row_lens_dev.data_ptr()),
                        eng, 'set_row_prefixes')
         self._trie_setup(lib, sl)
         if uniforms is not None and sp.mode == _lib.SEARCH_BEAM:
@@ -611,8 +623,10 @@ class GitB200CaptioningModel(nn.Module):
             _lib.check(lib.gitb200_set_beam_sampling(eng, uniforms.data_ptr(), int(uniforms.shape[0]), int(uniforms.shape[1]),
                                                      float(self.decoder.temperature), top_k, top_p), eng, 'set_beam_sampling')
         elif uniforms is not None:
-            _lib.check(lib.gitb200_set_sampling(eng, uniforms.data_ptr(), int(uniforms.shape[0]), B,
+            _lib.check(lib.gitb200_set_sampling(eng, uniforms.data_ptr(), int(uniforms.shape[0]), S,
                                                 float(search_param.get('temperature', 1))), eng, 'set_sampling')
+        if n_seq > 1:
+            _lib.check(lib.gitb200_set_sequences_per_image(eng, n_seq), eng, 'set_sequences_per_image')
         _lib.check(lib.gitb200_generate_async(
             eng, x.data_ptr(), B, frames, prefix.data_ptr() if prefix is not None else None, P,
             ctypes.byref(sp), forced.data_ptr() if forced is not None else None, tokens.data_ptr(),
@@ -696,7 +710,8 @@ class GitB200CaptioningModel(nn.Module):
 
     def _sampling_setup(self, search_param, sp, B, dev):
         """search_param of the reference's decoder.search (layers/decoder.py:224-232, 1083-1092) -> the uniforms the engine
-        draws with (None: a deterministic search)."""
+        draws with (None: a deterministic search).  B counts sequences: submit takes num_return_sequences out first and
+        passes B * n (a num_return_sequences above 1 that reaches this point raises)."""
         if not search_param:
             return None
         if isinstance(self.decoder, GeneratorWithBeamSearch):
@@ -871,6 +886,13 @@ class GitB200CaptioningModel(nn.Module):
         _lib.check(lib.gitb200_decode_step(self._engine, tokens.data_ptr(), bi.data_ptr() if bi is not None else None,
                                            rows, int(pos), logits.data_ptr(), stream), self._engine, 'decode_step')
         return logits
+
+
+def _sequences_per_image(n):
+    """The num_return_sequences of a search_param (reference layers/decoder.py:229-237, 1091-1096): an int >= 1."""
+    if isinstance(n, bool) or not isinstance(n, numbers.Integral) or int(n) < 1:
+        raise ValueError('num_return_sequences must be an integer >= 1 (got %r)' % (n,))
+    return int(n)
 
 
 def get_git_model(tokenizer, param):

@@ -62,8 +62,8 @@ enum { GITB200_F32 = 0, GITB200_BF16 = 1, GITB200_I64 = 2 };
 int gitb200_create(const gitb200_config* cfg, int device, gitb200_engine** out);
 void gitb200_destroy(gitb200_engine* h);
 const char* gitb200_last_error(const gitb200_engine* h);
-/* ABI version of the library (bumped on any signature change): 11 (gitb200_set_beam_sampling, gitb200_op_beam_sample);
- * 10 added gitb200_op_gemm_ex, gitb200_op_layernorm_ex and gitb200_op_lse_combine; 9 added gitb200_score and gitb200_op_text_attention. */
+/* ABI version of the library (bumped on any signature change): 12 (gitb200_set_sequences_per_image); 11 added
+ * gitb200_set_beam_sampling and gitb200_op_beam_sample; 10 added gitb200_op_gemm_ex, gitb200_op_layernorm_ex and gitb200_op_lse_combine; 9 added gitb200_score and gitb200_op_text_attention. */
 int gitb200_abi_version(void);
 
 /* Replaces: torch_common.load_state_dict -> module parameters           torch_common.py:93-145.
@@ -105,9 +105,9 @@ int gitb200_set_input_size(gitb200_engine* h, int height, int width);
  * and frames must be 0 or 1.  Image b has L_b = (H_b / patch) * (W_b / patch) + 1 tokens in a slot of L_max = max L_b
  * rows: row b of the results is what a batch-1 call with that image alone returns.  The greedy decode steps of such a
  * call run on the kernel chain (use_mega does not apply).  gitb200_set_input_size is left as it was.
- * Inputs of the next call only (this one, gitb200_set_row_prefixes, gitb200_set_sampling, gitb200_set_beam_sampling): the
- * next call that can use them takes them at entry, right after its in-flight check -- gitb200_encode and gitb200_score take
- * the image sizes, a gitb200_generate* call takes all four -- and they are gone from the engine whether that call succeeds or fails. */
+ * Inputs of the next call only (this one, gitb200_set_row_prefixes, gitb200_set_sampling, gitb200_set_beam_sampling,
+ * gitb200_set_sequences_per_image): the next call that can use them takes them at entry, right after its in-flight check --
+ * gitb200_encode and gitb200_score take the image sizes, a gitb200_generate* call takes all five -- and they are gone from the engine whether that call succeeds or fails. */
 int gitb200_set_image_sizes(gitb200_engine* h, const int32_t* hw_host, int n);
 
 /* Replaces: visual_projection + the image rows of BertEncoderAsDecoder, computed once (KV cache)
@@ -212,6 +212,17 @@ int gitb200_set_sampling(gitb200_engine* h, const float* uniforms_dev, int steps
  * synchronous generate call) fails naming its step and row.  The buffer must stay valid until the call has finished. */
 int gitb200_set_beam_sampling(gitb200_engine* h, const float* uniforms_dev, int steps, int rows, float temperature,
                               int top_k, float top_p);
+
+/* Replaces: the num_return_sequences argument of the three searches   layers/decoder.py:232-237, 1093-1096,
+ * trie_decoder.py:51-55, for the NEXT generate call, which takes it as gitb200_set_image_sizes describes: that call runs
+ * n >= 1 sequences for each of its `batch` images, in image-major order (sequence b * n + i belongs to image b), each
+ * searching independently.  Every image is encoded and its K/V cached once; its n sequences read that one copy.  The
+ * call's other per-row arguments count sequences, not images: the rows of gitb200_set_row_prefixes and of the sampling
+ * uniforms (batch * n, or batch * n * beam_size for beam sampling), forced_dev [batch * n, max_steps], tokens_out
+ * [batch * n, max_steps], logprobs_out [batch * n] and step_logits [steps, batch * n (* beam_size), vocab].  Each
+ * sequence's result is bit for bit what the call with every image repeated n times returns (greedy steps without the
+ * one-kernel step: a call with n > 1 runs on the kernel chain).  n = 1 is the call without it. */
+int gitb200_set_sequences_per_image(gitb200_engine* h, int n);
 
 /* Number of kernels the engine launched since creation (bench.py's gpu_launches). */
 int64_t gitb200_launch_count(const gitb200_engine* h);
