@@ -183,6 +183,7 @@ struct gitb200_engine {
   DevBuf beam_ws;                                           // beam-search bookkeeping (search.cuh)
   BeamState beam_s{};                                       // ... as the last beam generate carved it (gitb200_debug_read)
   int beam_B = 0, beam_max_steps = 0;                       // 0: the last prefill was not a beam generate
+  int beam_cand = 0;                                        // row stride of beam_s's candidate arrays (beam_cand_capacity)
   DevBuf sc_kv, sc_tgt, sc_part, sc_loss, sc_valid, sc_index;   // caption scoring: one layer's text K/V, LM-head targets /
                                                                // statistics, per-row losses, op image_index
   DevBuf sel_ws;                                            // greedy selection partials
@@ -639,7 +640,7 @@ static int launch_text_attention(gitb200_engine* h, const TextAttn& a, bool fp32
 // `items` (image, head) pairs.  The image K/V slice of one item is M rows of 128 B, staged in chunks of at most
 // kDecAttnChunk rows: two (K + V) staging buffers of one chunk per CTA, and at least two CTAs per SM (M = 257 in one piece
 // would be 131 KB per CTA = one 4-warp CTA per SM).  A uniform chunk is one TMA box.
-static DecAttnGeom dec_attn_geometry(int M, const int* lens, int n, int num_sms, int items) {
+static DecAttnGeom dec_attn_geometry(int M, const int* lens, int n, int num_sms, int items, int beam) {
   DecAttnGeom g;
   g.box_rows = g.chunk_rows = dec_attn_chunk_rows(M);
   if (lens != nullptr) {
@@ -651,7 +652,10 @@ static DecAttnGeom dec_attn_geometry(int M, const int* lens, int n, int num_sms,
     g.chunk_rows = (rows + kDecAttnRaggedBox - 1) / kDecAttnRaggedBox * kDecAttnRaggedBox;
   }
   g.smem = static_cast<size_t>(4) * g.chunk_rows * 128 + 128;
-  int per_sm = static_cast<int>((227 * 1024) / (g.smem + 8 * 1024));
+  // + an upper bound of the kernel's static shared memory and the 1 KB per-CTA reserve, which come to 7 KB at NQ 4 and
+  // 8 / 9 / 10 / 12 KB at NQ 5 .. 8 (ptxas)
+  const size_t fixed = static_cast<size_t>(std::max(8, beam + 4)) * 1024;
+  int per_sm = static_cast<int>((227 * 1024) / (g.smem + fixed));
   per_sm = std::max(1, std::min(per_sm, 4));
   g.grid = std::min(items, per_sm * num_sms);
   return g;
@@ -736,7 +740,15 @@ static int launch_decode_attention(gitb200_engine* h, const DecodeAttn& a, bool 
                       : launch_decode_attn_inst<3, false>(h, p, grid, smem, a.pdl, st, tk, tv);
     case 4: return rg ? launch_decode_attn_inst<4, true>(h, p, grid, smem, a.pdl, st, tk, tv)
                       : launch_decode_attn_inst<4, false>(h, p, grid, smem, a.pdl, st, tk, tv);
-    default: return fail(h, "decode: beam size %d not supported (1 .. 4)", a.beam);
+    case 5: return rg ? launch_decode_attn_inst<5, true>(h, p, grid, smem, a.pdl, st, tk, tv)
+                      : launch_decode_attn_inst<5, false>(h, p, grid, smem, a.pdl, st, tk, tv);
+    case 6: return rg ? launch_decode_attn_inst<6, true>(h, p, grid, smem, a.pdl, st, tk, tv)
+                      : launch_decode_attn_inst<6, false>(h, p, grid, smem, a.pdl, st, tk, tv);
+    case 7: return rg ? launch_decode_attn_inst<7, true>(h, p, grid, smem, a.pdl, st, tk, tv)
+                      : launch_decode_attn_inst<7, false>(h, p, grid, smem, a.pdl, st, tk, tv);
+    case 8: return rg ? launch_decode_attn_inst<8, true>(h, p, grid, smem, a.pdl, st, tk, tv)
+                      : launch_decode_attn_inst<8, false>(h, p, grid, smem, a.pdl, st, tk, tv);
+    default: return fail(h, "decode: beam size %d not supported (1 .. 8)", a.beam);
   }
 }
 
@@ -1529,7 +1541,7 @@ static int step_layers(gitb200_engine* h, cudaStream_t st, const long long* toke
 // Decode-attention geometry of the last prefill (dec_attn_geometry) and the step chain's counters.
 static int set_decode_geometry(gitb200_engine* h) {
   h->attn_geom = dec_attn_geometry(h->cur_M, h->cur_img.ragged ? h->cur_img.lens.data() : nullptr, h->cur_B, h->num_sms,
-                                   h->cur_B * h->cur_seqs * h->cfg.dec_heads);
+                                   h->cur_B * h->cur_seqs * h->cfg.dec_heads, h->cur_beam);
   CK(h->chain.ensure(256));
   CK(cudaMemset(h->chain.p, 0, 256));
   return 0;

@@ -25,8 +25,11 @@
 
 namespace gitb200 {
 
-constexpr int kMaxBeam = 4;
-constexpr int kMaxCand = 2 * kMaxBeam;  // per_node_beam_size * beam
+// Candidate capacity (per_node_beam_size * beam, per_node 2): the per-row lists, the row stride of BeamState's candidate
+// arrays and the merge width are compile-time.  Two instantiations: 8 for beams 2 .. 4, 16 for beams 5 .. 8.  The 16-entry
+// beam_row_topk_kernel takes several times as long per launch (DESIGN.md §6), so beams 2 .. 4 keep the 8-entry one.
+constexpr int kMaxBeam = 8;
+__host__ __device__ constexpr int beam_cand_capacity(int beam) { return beam <= 4 ? 8 : 16; }
 
 __global__ void init_src_row_kernel(int* src, int rows, int T_alloc) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -44,8 +47,8 @@ __global__ void reorder_src_row_kernel(const int* old_src, int* new_src, const i
 struct BeamState {
   // all arrays live in one engine-owned buffer; see beam_state_bytes()
   float* beam_scores;     // [rows]
-  float* cand_val;        // [rows, kMaxCand]  row-local top candidates: logit - lse + beam_score
-  int* cand_idx;          // [rows, kMaxCand]  vocabulary index
+  float* cand_val;        // [rows, kCand]  row-local top candidates: logit - lse + beam_score (kCand: beam_cand_capacity)
+  int* cand_idx;          // [rows, kCand]  vocabulary index
   long long* ids[2];      // [rows, max_steps] token history ping-pong (input_ids)
   int* src[2];            // [rows, T_alloc] text-KV indirection ping-pong
   int* cur;               // [1] which of ids/src is current
@@ -86,22 +89,23 @@ __device__ __forceinline__ float beam_length_norm(int length, float lp) {
   return powf(5.0f + static_cast<float>(length), lp) / powf(6.0f, lp);
 }
 
-// Sorted candidate list of kMaxCand entries in registers (descending value, ascending index on exact ties).  Every access is
+// Sorted candidate list of kCand entries in registers (descending value, ascending index on exact ties).  Every access is
 // statically indexed: indexing the arrays with a runtime position puts them in local memory, which made this kernel
 // several times slower.
+template <int kCand>
 struct TopList {
-  float v[kMaxCand];
-  int i[kMaxCand];
+  float v[kCand];
+  int i[kCand];
   __device__ __forceinline__ void init() {
 #pragma unroll
-    for (int k = 0; k < kMaxCand; ++k) { v[k] = -INFINITY; i[k] = 0x7fffffff; }
+    for (int k = 0; k < kCand; ++k) { v[k] = -INFINITY; i[k] = 0x7fffffff; }
   }
   static __device__ __forceinline__ bool before(float va, int ia, float vb, int ib) { return va > vb || (va == vb && ia < ib); }
   __device__ __forceinline__ void push(float val, int idx) {          // insert if it beats the last entry, keep sorted
-    if (!before(val, idx, v[kMaxCand - 1], i[kMaxCand - 1])) return;
-    v[kMaxCand - 1] = val; i[kMaxCand - 1] = idx;
+    if (!before(val, idx, v[kCand - 1], i[kCand - 1])) return;
+    v[kCand - 1] = val; i[kCand - 1] = idx;
 #pragma unroll
-    for (int k = kMaxCand - 1; k > 0; --k) {
+    for (int k = kCand - 1; k > 0; --k) {
       if (before(v[k], i[k], v[k - 1], i[k - 1])) {
         const float tv = v[k]; v[k] = v[k - 1]; v[k - 1] = tv;
         const int ti = i[k]; i[k] = i[k - 1]; i[k - 1] = ti;
@@ -111,7 +115,8 @@ struct TopList {
 };
 
 // One CTA per row: lse = logsumexp(z), then the row's top-NC values of (z - lse + beam_score[row]).  One pass over the
-// logits (online max / sum-exp and a sorted top-8 list per thread), then lists merged by shuffles and through shared memory.
+// logits (online max / sum-exp and a sorted top-kCand list per thread), then lists merged by shuffles and through shared memory.
+template <int kCand>
 __global__ void __launch_bounds__(kRowThreads) beam_row_topk_kernel(const BeamParams p) {
   griddep_launch();
   StepState* st = p.state;
@@ -122,7 +127,7 @@ __global__ void __launch_bounds__(kRowThreads) beam_row_topk_kernel(const BeamPa
   const float* z = p.logits + static_cast<long long>(row) * p.V;
   if (float* dst = step_logits_row(p.step_logits, st->step, gridDim.x, row, p.V))
     for (int i = tid; i < p.V; i += blockDim.x) dst[i] = z[i];   // a kRowThreads stride changes the kernel's code
-  TopList top;
+  TopList<kCand> top;
   top.init();
   float mx = -INFINITY, sum = 0.f;
   for (int i0 = tid; i0 < p.V; i0 += 8 * kRowThreads) {       // 8 independent loads in flight per thread
@@ -146,20 +151,20 @@ __global__ void __launch_bounds__(kRowThreads) beam_row_topk_kernel(const BeamPa
     const float mn = fmaxf(mx, m_o);
     sum = sum * ((mx == -INFINITY) ? 0.f : __expf(mx - mn)) + s_o * ((m_o == -INFINITY) ? 0.f : __expf(m_o - mn));
     mx = mn;
-    float pv[kMaxCand];
-    int pi[kMaxCand];
+    float pv[kCand];
+    int pi[kCand];
 #pragma unroll
-    for (int k = 0; k < kMaxCand; ++k) { pv[k] = __shfl_xor_sync(0xffffffffu, top.v[k], o); pi[k] = __shfl_xor_sync(0xffffffffu, top.i[k], o); }
+    for (int k = 0; k < kCand; ++k) { pv[k] = __shfl_xor_sync(0xffffffffu, top.v[k], o); pi[k] = __shfl_xor_sync(0xffffffffu, top.i[k], o); }
 #pragma unroll
-    for (int k = 0; k < kMaxCand; ++k) top.push(pv[k], pi[k]);
+    for (int k = 0; k < kCand; ++k) top.push(pv[k], pi[k]);
   }
   __shared__ float s_m[kRowWarps], s_s[kRowWarps];
-  __shared__ float s_cv[kRowWarps][kMaxCand];
-  __shared__ int s_ci[kRowWarps][kMaxCand];
+  __shared__ float s_cv[kRowWarps][kCand];
+  __shared__ int s_ci[kRowWarps][kCand];
   if (lane == 0) {
     s_m[warp] = mx; s_s[warp] = sum;
 #pragma unroll
-    for (int k = 0; k < kMaxCand; ++k) { s_cv[warp][k] = top.v[k]; s_ci[warp][k] = top.i[k]; }
+    for (int k = 0; k < kCand; ++k) { s_cv[warp][k] = top.v[k]; s_ci[warp][k] = top.i[k]; }
   }
   __syncthreads();
   if (tid == 0) {
@@ -168,16 +173,16 @@ __global__ void __launch_bounds__(kRowThreads) beam_row_topk_kernel(const BeamPa
       sum = sum * ((mx == -INFINITY) ? 0.f : __expf(mx - mn)) + s_s[w] * ((s_m[w] == -INFINITY) ? 0.f : __expf(s_m[w] - mn));
       mx = mn;
 #pragma unroll
-      for (int k = 0; k < kMaxCand; ++k) top.push(s_cv[w][k], s_ci[w][k]);
+      for (int k = 0; k < kCand; ++k) top.push(s_cv[w][k], s_ci[w][k]);
     }
     const float log_sum = logf(sum);
     const float bs = p.s.beam_scores[row];
 #pragma unroll
-    for (int k = 0; k < kMaxCand; ++k) {
+    for (int k = 0; k < kCand; ++k) {
       if (k < NC) {
         // log_softmax (x - max - log(sum exp(x - max))) + beam score (reference :1169-1172)
-        p.s.cand_val[row * kMaxCand + k] = ((top.v[k] - mx) - log_sum) + bs;
-        p.s.cand_idx[row * kMaxCand + k] = top.i[k];
+        p.s.cand_val[row * kCand + k] = ((top.v[k] - mx) - log_sum) + bs;
+        p.s.cand_idx[row * kCand + k] = top.i[k];
       }
     }
   }
@@ -306,6 +311,7 @@ __device__ RadixStop radix_descend(const float* s, int V, float want, unsigned i
   return r;
 }
 
+template <int kCand>   // the row stride of the candidate arrays
 __global__ void __launch_bounds__(kRowThreads) beam_sample_kernel(const BeamParams p) {
   griddep_launch();
   StepState* st = p.state;
@@ -432,14 +438,15 @@ __global__ void __launch_bounds__(kRowThreads) beam_sample_kernel(const BeamPara
     return;
   }
   const float lse = logf(total1), bs = p.s.beam_scores[row];
-  p.s.cand_val[row * kMaxCand] = ((srow[t1] - m) - lse) + bs;
-  p.s.cand_idx[row * kMaxCand] = t1;
-  p.s.cand_val[row * kMaxCand + 1] = ((srow[t2] - m) - lse) + bs;
-  p.s.cand_idx[row * kMaxCand + 1] = t2;
+  p.s.cand_val[row * kCand] = ((srow[t1] - m) - lse) + bs;
+  p.s.cand_idx[row * kCand] = t1;
+  p.s.cand_val[row * kCand + 1] = ((srow[t2] - m) - lse) + bs;
+  p.s.cand_idx[row * kCand + 1] = t2;
   if (p.smp.kept != nullptr) p.smp.kept[row] = n_kept;
 }
 
 // One thread block per image (32 threads; the bookkeeping itself is sequential like the reference's loop).
+template <int kCand>
 __global__ void __launch_bounds__(32) beam_update_kernel(const BeamParams p) {
   griddep_launch();
   StepState* st = p.state;
@@ -453,12 +460,12 @@ __global__ void __launch_bounds__(32) beam_update_kernel(const BeamParams p) {
   long long* ids_new = p.s.ids[cur ^ 1];
   const int* src_old = p.s.src[cur];
   int* src_new = p.s.src[cur ^ 1];
-  __shared__ float m_val[kMaxCand];
-  __shared__ int m_word[kMaxCand];
-  __shared__ int m_beam[kMaxCand];
-  __shared__ int n_row[kMaxBeam];   // next beams: source row (global)
-  __shared__ int n_word[kMaxBeam];
-  __shared__ float n_score[kMaxBeam];
+  __shared__ float m_val[kCand];
+  __shared__ int m_word[kCand];
+  __shared__ int m_beam[kCand];
+  __shared__ int n_row[kCand / 2];   // next beams: source row (global)
+  __shared__ int n_word[kCand / 2];
+  __shared__ float n_score[kCand / 2];
   const bool in_prefix = (p.row_prefix != nullptr) && cur_len < p.row_prefix_lens[b];
   if (lane == 0 && in_prefix) {
     // the image is still inside its prefix: every beam takes the next prefix token, scores and histories stay as they are
@@ -477,14 +484,14 @@ __global__ void __launch_bounds__(32) beam_update_kernel(const BeamParams p) {
       top = -INFINITY;
       for (int c = 0; c < NC; ++c) {
         const int r = b * beam + c / p.per_node;
-        m_val[c] = p.s.cand_val[r * kMaxCand + c % p.per_node];
-        m_word[c] = p.s.cand_idx[r * kMaxCand + c % p.per_node];
+        m_val[c] = p.s.cand_val[r * kCand + c % p.per_node];
+        m_word[c] = p.s.cand_idx[r * kCand + c % p.per_node];
         m_beam[c] = c % beam;
         top = fmaxf(top, m_val[c]);
       }
     } else {
       // merge the `beam` row lists into the image's top-NC, ordered by (value desc, flat index asc)
-      int ptr[kMaxBeam];
+      int ptr[kCand / 2];
       for (int k = 0; k < beam; ++k) ptr[k] = 0;
       for (int c = 0; c < NC; ++c) {
         int best = -1;
@@ -493,12 +500,12 @@ __global__ void __launch_bounds__(32) beam_update_kernel(const BeamParams p) {
         for (int k = 0; k < beam; ++k) {
           if (ptr[k] >= NC) continue;
           const int r = b * beam + k;
-          const float v = p.s.cand_val[r * kMaxCand + ptr[k]];
-          const long long flat = static_cast<long long>(k) * V + p.s.cand_idx[r * kMaxCand + ptr[k]];
+          const float v = p.s.cand_val[r * kCand + ptr[k]];
+          const long long flat = static_cast<long long>(k) * V + p.s.cand_idx[r * kCand + ptr[k]];
           if (best < 0 || v > bv || (v == bv && flat < bflat)) { best = k; bv = v; bflat = flat; }
         }
         m_val[c] = bv;
-        m_word[c] = p.s.cand_idx[(b * beam + best) * kMaxCand + ptr[best]];
+        m_word[c] = p.s.cand_idx[(b * beam + best) * kCand + ptr[best]];
         m_beam[c] = best;
         ++ptr[best];
       }

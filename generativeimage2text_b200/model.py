@@ -40,7 +40,8 @@ class AutoRegressiveBeamSearch(object):
 
 class GeneratorWithBeamSearch(object):
     """Search configuration mirroring reference layers/decoder.py:1056-1081 (the shipped default:
-    beam 4, per-node 2, length_penalty 0.6, model.py:34-40).  The constructor takes temperature 1 only; sampled beam search
+    beam 4, per-node 2, length_penalty 0.6, model.py:34-40); the engine runs beam sizes 2 .. 8 with per-node 2.  The
+    constructor takes temperature 1 only; sampled beam search
     (search_param={'do_sample': True, ...}) divides the logits by the `temperature` attribute, the value the reference's
     search reads (layers/decoder.py:1097, 1140-1142), so `decoder.temperature = 0.7` sets it."""
 

@@ -51,7 +51,7 @@ typedef struct gitb200_search {
   int32_t mode;            /* GREEDY = AutoRegressiveBeamSearch(beam 1, per-node 1)  layers/decoder.py:208-440
                               BEAM   = GeneratorWithBeamSearch                        layers/decoder.py:1056-1341 */
   int32_t max_steps;       /* output length cap incl. start tokens (40 in BASELINE.json; 1024 stock) */
-  int32_t beam_size;       /* 4                                                       model.py:38  */
+  int32_t beam_size;       /* 4 (BEAM: 2 .. 8)                                        model.py:38  */
   int32_t per_node_beam;   /* 2                                                       layers/decoder.py:1062 */
   float length_penalty;    /* 0.6                                                     model.py:39  */
 } gitb200_search;
@@ -112,12 +112,12 @@ int gitb200_set_image_sizes(gitb200_engine* h, const int32_t* hw_host, int n);
 
 /* Replaces: visual_projection + the image rows of BertEncoderAsDecoder, computed once (KV cache)
  *                                      layers/decoder.py:535, 92-174; layers/bert/modeling_bert.py:92-334.
- * Uses the features of the last gitb200_encode. vproj_out_dev: fp32 [B, M, 768] or NULL. */
+ * Uses the features of the last gitb200_encode; beam 1 .. 8. vproj_out_dev: fp32 [B, M, 768] or NULL. */
 int gitb200_prefill(gitb200_engine* h, int batch, int beam, float* vproj_out_dev, void* stream);
 
 /* Replaces: CaptioningModel.decoding_step (one new token per row)       layers/decoder.py:1013-1054.
  * tokens_dev: int64 [rows] newest token of each row (rows = batch*beam), appended at text position
- * `pos`; beam_idx_dev (int32 [rows], may be NULL) re-orders the text KV cache first
+ * `pos` (rows and beam as the last gitb200_prefill: beam 1 .. 8); beam_idx_dev (int32 [rows], may be NULL) re-orders the text KV cache first
  * (layers/decoder.py:1231).  logits_out_dev: fp32 [rows, vocab] raw last-position logits. */
 int gitb200_decode_step(gitb200_engine* h, const int64_t* tokens_dev, const int32_t* beam_idx_dev, int rows,
                         int pos, float* logits_out_dev, void* stream);
@@ -388,8 +388,9 @@ int gitb200_preproc_coeffs(int in_size, int out_size, int32_t* ksize_out, int32_
  *   "beam_scores" fp32 [rows]: the running beam scores, after a beam generate;
  *   "beam_hyp"    [4][batch] 4-byte words, after a beam generate: done (int32), hyp_len (int32, 0 = no hypothesis),
  *                 hyp_score (fp32, length-normalised), worst_score (fp32).
- *   "beam_cand"   [2][rows][8] 4-byte words, after a beam generate: the last step's per-row candidate list, scores
- *                 (fp32: log-softmax + beam score) then token ids (int32); the first 2 * beam entries of a row are valid.
+ *   "beam_cand"   [2][rows][C] 4-byte words, after a beam generate: the last step's per-row candidate list, scores
+ *                 (fp32: log-softmax + beam score) then token ids (int32); C = 8 for beam sizes 2 .. 4 and 16 for 5 .. 8;
+ *                 the first 2 * beam entries of a row are valid.
  * Returns bytes copied or -1. */
 long long gitb200_debug_read(gitb200_engine* h, const char* name, void* out_host, long long max_bytes);
 /* Debug aid: in-situ timeline of the decode-step kernels. enable != 0 arms it; enable == 0 copies up to
